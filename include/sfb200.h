@@ -80,6 +80,7 @@ int sfb_tmap_nhwc(void* out128, const void* base, uint32_t n, uint32_t h, uint32
 enum sfb_gemm_a_mode {
     SFB_A_MATRIX = 0,  /* A is [M, K] row-major (linear layers, 1x1 convolutions) */
     SFB_A_CONV3X3 = 1, /* A is an NHWC image; K = 9 * cin, padding 1, stride 1 or 2 */
+    /* (SFB_A_DOWNCONV3X3 = 5, below: the stride-2 variant with padding after the image only) */
     /* nearest-2x upsample followed by a 3x3 convolution, computed on the LOW-resolution image
      * without materialising the upsampled tensor: output pixel (2y+py, 2x+px) only sees a 2x2
      * neighbourhood of the source, so each of the 4 output phases (py, px) is a 2x2 convolution
@@ -107,6 +108,14 @@ enum sfb_gemm_a_mode {
      * (/root/reference/src/sfast/jit/passes/triton_passes.py:68-88,
      *  src/sfast/triton/ops/group_norm.py:272-320) in front of cudnn_convolution_bias(_add). */
     SFB_A_CONV3X3_GN = 4,
+    /* 3x3 convolution, stride 2, zero padding of ONE row and ONE column AFTER the image and none before
+     * (diffusers' Downsample2D with padding=0, the VAE encoder's downsampler: F.pad(x, (0, 1, 0, 1))
+     * then a pad-0 stride-2 conv): output pixel (i, j) reads input rows 2i..2i+2 and columns 2j..2j+2.
+     * A is the INPUT image through sfb_tmap_nhwc with stride 2 over [n, 2 * img_h, 2 * img_w, cin];
+     * the last tap lands on row / column 2 * img_h / 2 * img_w, past the image, which TMA zero-fills.
+     * img_* are the OUTPUT dims; K = 9 * cin (cin % 64 == 0), conv_stride must be 2, no rowbias;
+     * box, split-K and epilogue rules as for SFB_A_CONV3X3. */
+    SFB_A_DOWNCONV3X3 = 5,
 };
 
 enum sfb_epilogue {
@@ -320,7 +329,8 @@ int sfb_small_linear(const sfb_small_linear_params* p, sfb_stream_t stream);
  * conv_in:  x NCHW [n, cin<=8, h, w] 16-bit  -> y NHWC [n, h, w, cout] (channel pitch ldy)
  * conv_out: x NHWC [n, h, w, cin] (pitch ldx) -> y NCHW [n, cout<=8, h, w] 16-bit
  * conv_in  w: 16-bit [3, 3, cin, cout] (tap-major, cout contiguous);
- * conv_out w: 16-bit [cout, 3, 3, cin]; bias fp32. */
+ * conv_out w: 16-bit [cout, 3, 3, cin]; bias fp32.  Both stage the whole weight in shared memory:
+ * conv_in up to 48 KB, conv_out up to 227 KB (e.g. the VAE encoder's 512 -> 8 conv_out, 72 KB). */
 /* im2col of the first convolution: x NCHW [n, cin<=7, h, w] 16-bit -> a [n*h*w, 64] 16-bit with
  * a[p, (kh*3+kw)*cin + c] and zero padding up to 64; feeds sfb_gemm (K = 64). */
 int sfb_im2col_in(const void* x, void* a, int32_t n, int32_t h, int32_t wd, int32_t cin,

@@ -288,9 +288,11 @@ __device__ __forceinline__ void tap_offset(const GemmArgs& a, const ATile& t, in
         dw = 0;
         dh = tap - 1;
     } else {
+        // SFB_A_DOWNCONV3X3 pads only after the last row / column: its taps start at the pixel itself
+        const int org = a.a_mode == SFB_A_DOWNCONV3X3 ? 0 : 1;
         const int kh = tap / 3, kw = tap - kh * 3;
-        dw = kw - 1;
-        dh = kh - 1;
+        dw = kw - org;
+        dh = kh - org;
     }
 }
 
@@ -1133,6 +1135,10 @@ extern "C" int sfb_gemm(const sfb_gemm_params* p, sfb_stream_t stream_) {
     const bool upconv = p->a_mode == SFB_A_UPCONV2X;
     const bool tconv = p->a_mode == SFB_A_CONV3X1;
     const bool gnconv = p->a_mode == SFB_A_CONV3X3_GN;
+    const bool downconv = p->a_mode == SFB_A_DOWNCONV3X3;
+    if (downconv && (p->conv_stride != 2 || p->rowbias))
+        return fail(SFB_ERR_INVALID, "sfb_gemm: SFB_A_DOWNCONV3X3 needs stride 2 and no rowbias (stride=%d)",
+                    p->conv_stride);
     if (gnconv) {
         // 16 x 8 pixel patches, halo tile transformed in shared memory (tmap_a box = [64, 10, 18, 1])
         if (!p->gn_scale_shift) return fail(SFB_ERR_INVALID, "sfb_gemm: SFB_A_CONV3X3_GN needs gn_scale_shift");
@@ -1143,7 +1149,7 @@ extern "C" int sfb_gemm(const sfb_gemm_params* p, sfb_stream_t stream_) {
         a.gn_ab = p->gn_scale_shift;
         a.gn_silu = p->gn_silu ? 1 : 0;
     }
-    if (p->a_mode == SFB_A_CONV3X3 || upconv || tconv || gnconv) {
+    if (p->a_mode == SFB_A_CONV3X3 || upconv || tconv || gnconv || downconv) {
         if (p->cin <= 0 || p->cin % BK || p->K != (upconv ? 4 : (tconv ? 3 : 9)) * p->cin)
             return fail(SFB_ERR_INVALID, "sfb_gemm: conv cin=%d K=%d", p->cin, p->K);
         const int box_w = p->box_w > 0 ? p->box_w : p->img_w;

@@ -571,7 +571,20 @@ extern "C" int sfb_conv_out(const void* x, const void* w, const float* bias, voi
     if (!x || !w || !y || cout <= 0 || cout > 8 || cin % 8 || ldx % 8)
         return fail(SFB_ERR_INVALID, "conv_out: unsupported geometry cin=%d cout=%d", cin, cout);
     const size_t smem = (size_t)9 * cin * cout * 2;
-    if (smem > 48 * 1024) return fail(SFB_ERR_INVALID, "conv_out: weights exceed 48 KB of shared memory");
+    // sm_90's per-block opt-in limit: the VAE encoder's conv_out (512 -> 8, 72 KB) needs more than the
+    // default 48 KB; launches within 48 KB (the decoder's 128 -> 3) never touch the attribute
+    constexpr size_t kSmemOptin = 227 * 1024;
+    if (smem > kSmemOptin) return fail(SFB_ERR_INVALID, "conv_out: weights exceed 227 KB of shared memory");
+    if (smem > 48 * 1024) {
+        static PerDeviceOnce attr_once;
+        bool& attr_set = attr_once.flag();
+        if (!attr_set) {
+            cudaError_t err = cudaFuncSetAttribute(conv_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   (int)kSmemOptin);
+            if (err != cudaSuccess) return fail(SFB_ERR_CUDA, "conv_out: smem attribute: %s", cudaGetErrorString(err));
+            attr_set = true;
+        }
+    }
     ConvEdgeArgs a{reinterpret_cast<const uint16_t*>(x), reinterpret_cast<const uint16_t*>(w), bias,
                    reinterpret_cast<uint16_t*>(y), n, h, wd, cin, cout, ldx, dtype};
     const int total = n * h * wd;

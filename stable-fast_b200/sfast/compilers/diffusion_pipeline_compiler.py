@@ -111,10 +111,13 @@ def compile_unet(m, config):
 
 
 def compile_vae(m, config):
-    """Replace ``m.decode`` with the H100-native VAE decoder (reference `compile_vae`, :154-190, which
-    wraps the sub-modules in auto-trace hooks); `encode` stays eager.  A VAE without a `decode`
-    method, or one on a non-sm_90 device, is returned unchanged with a warning (the reference, too,
-    only hooks what it can trace)."""
+    """Replace ``m.decode`` and ``m.encode`` with the H100-native VAE decoder and encoder (reference
+    `compile_vae`, :154-190, which wraps the sub-modules in auto-trace hooks).  Both share one packed
+    copy of the weights.  `encode` is replaced only where the module has one (img2img and inpainting
+    call it every time).  A VAE without post_quant_conv (SVD's AutoencoderKLTemporalDecoder, whose
+    decode takes num_frames) keeps its own decode.  fp32 calls (force_upcast) and diffusers' tiled
+    encode stay on the module's eager path.  A VAE without a `decode` method is returned unchanged
+    with a warning (the reference, too, only hooks what it can trace)."""
     from sfast_b200.runtime import compile_vae_module, require_sm90
     if not hasattr(m, 'decode') or not hasattr(m, 'config'):
         logger.warning('sfast (H100 build): VAE without decode()/config is left on its eager path')

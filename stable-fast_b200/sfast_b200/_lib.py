@@ -12,7 +12,7 @@ LIB_PATH = os.environ.get("SFB_LIB_PATH") or os.path.join(_HERE, "libsfb200.so")
 
 ABI_VERSION = 4  # SFB_ABI_VERSION of include/sfb200.h
 SFB_F16, SFB_BF16 = 0, 1
-A_MATRIX, A_CONV3X3, A_UPCONV2X, A_CONV3X1, A_CONV3X3_GN = 0, 1, 2, 3, 4
+A_MATRIX, A_CONV3X3, A_UPCONV2X, A_CONV3X1, A_CONV3X3_GN, A_DOWNCONV3X3 = 0, 1, 2, 3, 4, 5
 ROW_IDX_DIV_MOD, ROW_IDX_TEMPORAL_CTX = 0, 1
 EPI_STORE, EPI_GEGLU, EPI_QKV, EPI_STORE_F32 = 0, 1, 2, 3
 ACT_NONE, ACT_QUICK_GELU, ACT_GELU = 0, 1, 2

@@ -11,7 +11,7 @@ import os
 import torch
 
 from . import _lib
-from ._lib import (A_CONV3X1, A_CONV3X3, A_CONV3X3_GN, A_MATRIX, A_UPCONV2X, EPI_GEGLU, EPI_QKV, EPI_STORE, AttnParams, GemmParams,
+from ._lib import (A_CONV3X1, A_CONV3X3, A_CONV3X3_GN, A_DOWNCONV3X3, A_MATRIX, A_UPCONV2X, EPI_GEGLU, EPI_QKV, EPI_STORE, AttnParams, GemmParams,
                    GnParams, LnParams, SmallLinearParams, TensorMap, check)
 
 BM, BN, BK = 128, 160, 64
@@ -240,6 +240,12 @@ def gemm_op(name, lib, *, M, N, K, dt, a_map=None, b_map=None, a=None, b=None, o
     p.a_mode = (A_UPCONV2X if up else (A_CONV3X1 if conv.get("temporal") else A_CONV3X3)) if conv else A_MATRIX
     if gn is not None:
         p.a_mode = A_CONV3X3_GN
+    if conv and conv.get("down"):
+        # the tensor map covers the input image, which the C side cannot see: output = input / 2 here
+        if a is not None and (a["h"], a["w"]) != (2 * conv["h"], 2 * conv["w"]):
+            raise ValueError(f"{name}: down-conv output {conv['h']}x{conv['w']} is not half of the input "
+                             f"{a['h']}x{a['w']}")
+        p.a_mode = A_DOWNCONV3X3
     p.M, p.N, p.K, p.dtype = M, N, K, dtype_code(dt)
     if conv:
         p.img_n, p.img_h, p.img_w = conv["n"], conv["h"], conv["w"]
@@ -524,6 +530,16 @@ def pack_upconv(w, dt):
                     c0 = (2 * ty + tx) * cin
                     out[r0:r0 + cout, c0:c0 + cin] = acc
     return out.to(dt).contiguous()
+
+
+def fold_pointwise_into_conv(w, b, w_pw, b_pw):
+    """A conv (w [c1, cin, kh, kw], b [c1]) followed by a 1x1 conv (w_pw [c2, c1, 1, 1], b_pw [c2]) as ONE
+    conv: W = W_pw . W, b = W_pw . b + b_pw, formed in fp32 (fp64 stays fp64) before any rounding."""
+    dt = torch.promote_types(w.dtype, torch.float32)
+    wq = w_pw.detach().to(dt).reshape(w_pw.shape[0], -1)
+    wf = torch.einsum("qo,ochw->qchw", wq, w.detach().to(dt))
+    bf = wq @ b.detach().to(dt) + b_pw.detach().to(dt)
+    return wf, bf
 
 
 def pack_conv_in(w, dt):

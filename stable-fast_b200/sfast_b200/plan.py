@@ -121,6 +121,15 @@ class PackedWeights:
         return self._get(("c3p", name), lambda: ops.pack_conv3x3(self._raw(name).to(self.device),
                                                                 self.dtype))
 
+    def conv3x3_pointwise(self, conv, pointwise):
+        """3x3 conv `conv` followed by the 1x1 conv `pointwise` (module prefixes) as one 3x3 conv
+        (ops.fold_pointwise_into_conv): (weight packed like conv3x3_plain, fp32 bias)."""
+        def build():
+            w, b = ops.fold_pointwise_into_conv(*(self._raw(f"{p}.{t}").to(self.device)
+                                                  for p in (conv, pointwise) for t in ("weight", "bias")))
+            return ops.pack_conv3x3(w, self.dtype), b.float().contiguous()
+        return self._get(("c3pw", conv, pointwise), build)
+
     def conv_in_matrix(self, name):
         """First conv as a GEMM operand: [cout, (kh, kw, cin)] zero-padded along K to 64."""
         def build():
@@ -396,7 +405,12 @@ class UNetPlan:
                                          groups=self.spec.groups, eps=eps, dt=self.dt))
         return x, dict(scale_shift=ab, silu=True)
 
-    def conv3x3(self, name, x: Act, wname, dst: Act, stride=1, rowbias=None, residual: Act = None, gn=None):
+    def conv3x3(self, name, x: Act, wname, dst: Act, stride=1, rowbias=None, residual: Act = None, gn=None,
+                down=False):
+        """`down`: diffusers' Downsample2D with padding=0 (the VAE encoder's) -- stride 2, one zero row and
+        column AFTER the image, none before (SFB_A_DOWNCONV3X3)."""
+        if down:
+            stride = 2
         wm = self.w.conv3x3(wname + ".weight")
         cout = wm.n
         ho, wo = x.h // stride, x.w // stride
@@ -411,7 +425,7 @@ class UNetPlan:
         kw = dict(a=adesc, b=wm, M=M, N=cout, K=9 * x.c, dt=self.dt,
                   out=dst.ptr, ldo=dst.ld, bias=self.w.f32(wname + ".bias"),
                   conv=dict(n=x.n, h=ho, w=wo, cin=x.c, stride=stride, box_n=box_n, box_h=box_h,
-                            box_w=box_w),
+                            box_w=box_w, down=down),
                   keep=(x.buf, dst.buf, wm))
         if rowbias is not None:
             kw.update(rowbias=rowbias[0], rows_per_img=ho * wo, ld_rowbias=rowbias[1])

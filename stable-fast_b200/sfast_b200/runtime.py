@@ -7,6 +7,7 @@ output is returned as a fresh clone, all under a per-object lock; unlike the ref
 timestep is always read from device memory inside the graph (never keyed by value,
 graphs.py:229-231).
 """
+import functools
 import logging
 import threading
 import time
@@ -254,48 +255,118 @@ class DecoderOutput(dict):
         return tuple(self.values())[k] if isinstance(k, int) else super().__getitem__(k)
 
 
-class CompiledVAEDecoder:
-    """`AutoencoderKL.decode(z, return_dict=True, generator=None)` on the native path."""
+class AutoencoderKLOutput(dict):
+    """Stand-in for diffusers' AutoencoderKLOutput (attribute, key and index access)."""
 
-    def __init__(self, config, state_dict_fn, eager_decode, enable_cuda_graph=True):
+    def __init__(self, latent_dist):
+        super().__init__(latent_dist=latent_dist)
+        self.latent_dist = latent_dist
+
+    def __getitem__(self, k):
+        return tuple(self.values())[k] if isinstance(k, int) else super().__getitem__(k)
+
+
+class DiagonalGaussianDistribution:
+    """Stand-in for diffusers' DiagonalGaussianDistribution over the encoder's moments [B, 2 * C, h, w]
+    (mean | log-variance along dim 1)."""
+
+    def __init__(self, parameters, deterministic=False):
+        self.parameters = parameters
+        self.mean, self.logvar = torch.chunk(parameters, 2, dim=1)
+        self.logvar = torch.clamp(self.logvar, -30.0, 20.0)
+        self.deterministic = deterministic
+        self.std = torch.exp(0.5 * self.logvar)
+        self.var = torch.exp(self.logvar)
+        if deterministic:
+            self.var = self.std = torch.zeros_like(self.mean)
+
+    def sample(self, generator=None):
+        # diffusers' randn_tensor: drawn in the moments' dtype on the generator's device when that is the
+        # CPU, else on the moments' device; one [1, ...] draw per generator when given a list
+        shape, dev, dt = tuple(self.mean.shape), self.parameters.device, self.parameters.dtype
+        g0 = generator[0] if isinstance(generator, (list, tuple)) else generator
+        rdev = torch.device("cpu") if g0 is not None and g0.device.type == "cpu" else dev
+        if isinstance(generator, (list, tuple)):
+            eps = torch.cat([torch.randn((1,) + shape[1:], generator=g, device=rdev, dtype=dt) for g in generator])
+        else:
+            eps = torch.randn(shape, generator=generator, device=rdev, dtype=dt)
+        return self.mean + self.std * eps.to(dev)
+
+    def mode(self):
+        return self.mean
+
+
+@functools.lru_cache(maxsize=None)
+def _latent_dist_classes():
+    """(AutoencoderKLOutput, DiagonalGaussianDistribution): diffusers' own where it imports."""
+    try:
+        from diffusers.models.autoencoders.vae import DiagonalGaussianDistribution as DGD  # type: ignore
+        from diffusers.models.modeling_outputs import AutoencoderKLOutput as Out  # type: ignore
+        return Out, DGD
+    except Exception:  # noqa: BLE001
+        return AutoencoderKLOutput, DiagonalGaussianDistribution
+
+
+def temporal_decoder(state_dict):
+    """True for a VAE whose decoder is not the 2-D `Decoder` the native path runs: SVD's
+    AutoencoderKLTemporalDecoder has no post_quant_conv and takes decode(z, num_frames=...)."""
+    return "post_quant_conv.weight" not in state_dict
+
+
+class CompiledVAE:
+    """`AutoencoderKL.decode(z, return_dict=True, generator=None)` and `encode(x, return_dict=True)` on the
+    native path.  Both share one packed copy of the weights, refreshed in place when the parameters'
+    version counters move, and one cache of plans + CUDA graphs keyed by (kind, B, H, W, dtype, device)."""
+
+    def __init__(self, module, eager_decode, eager_encode, enable_cuda_graph=True):
         from .vae_plan import vae_spec_from_config
-        self.spec = vae_spec_from_config(config)
-        self._state_dict_fn, self._eager = state_dict_fn, eager_decode
+        # eager_decode / eager_encode None: that entry is not compiled (it stays the module's own)
+        self.spec = vae_spec_from_config(module.config)
+        self._module, self._state_dict_fn = module, module.state_dict
+        self._eager, self._eager_encode = eager_decode, eager_encode
         self.enable_cuda_graph = enable_cuda_graph
         self._weights, self._param_refs, self._param_versions = None, None, None
         self._cached = {}
         self._lock = threading.Lock()
-        self._warned = False
+        self._warned = set()
 
-    def __call__(self, z, return_dict=True, generator=None):
+    def _warn_once(self, what, msg, *args):
+        if what not in self._warned:
+            logger.warning(msg, *args)
+            self._warned.add(what)
+
+    def _graphed(self, kind, plan_cls, x):
+        """Plan + graph of `kind` for x's shape (caller holds the lock and x's device is current)."""
+        if self._weights is None or self._weights.dtype != x.dtype or self._weights.device != x.device:
+            sd = self._state_dict_fn()
+            self._weights = PackedWeights(self.spec, sd, x.dtype, x.device)
+            self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
+            self._param_versions = [t._version for t in self._param_refs]
+            self._cached.clear()
+        elif [t._version for t in self._param_refs] != self._param_versions:
+            sd = self._state_dict_fn()
+            torch.cuda.current_stream().synchronize()
+            self._weights.refresh(sd)
+            self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
+            self._param_versions = [t._version for t in self._param_refs]
+        B, _, H, W = x.shape
+        key = (kind, B, H, W, x.dtype, x.device.index)
+        gp = self._cached.get(key)
+        if gp is None:
+            gp = _GraphedPlan(plan_cls(self._weights, B, H, W), self.enable_cuda_graph)
+            self._cached[key] = gp
+        return gp
+
+    def decode(self, z, return_dict=True, generator=None):
         from .vae_plan import VAEDecodePlan
         if z.dtype not in (torch.float16, torch.bfloat16):
             # e.g. SDXL's force_upcast fp32 VAE: the whole module stays on its own eager path
-            if not self._warned:
-                logger.warning("sfast (H100 build): VAE decode in %s is left on the module's eager path "
-                               "(the native decoder computes in fp16 / bf16)", z.dtype)
-                self._warned = True
+            self._warn_once("decode_dtype", "sfast (H100 build): VAE decode in %s is left on the module's eager "
+                            "path (the native decoder computes in fp16 / bf16)", z.dtype)
             return self._eager(z, return_dict=return_dict, generator=generator)
         require_sm90(z.device)
-        B, _, H, W = z.shape
         with self._lock, torch.cuda.device(z.device):
-            if self._weights is None or self._weights.dtype != z.dtype or self._weights.device != z.device:
-                sd = self._state_dict_fn()
-                self._weights = PackedWeights(self.spec, sd, z.dtype, z.device)
-                self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
-                self._param_versions = [t._version for t in self._param_refs]
-                self._cached.clear()
-            elif [t._version for t in self._param_refs] != self._param_versions:
-                sd = self._state_dict_fn()
-                torch.cuda.current_stream().synchronize()
-                self._weights.refresh(sd)
-                self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
-                self._param_versions = [t._version for t in self._param_refs]
-            key = (B, H, W, z.dtype, z.device.index)
-            gp = self._cached.get(key)
-            if gp is None:
-                gp = _GraphedPlan(VAEDecodePlan(self._weights, B, H, W), self.enable_cuda_graph)
-                self._cached[key] = gp
+            gp = self._graphed("decode", VAEDecodePlan, z)
             gp.plan.z_in.copy_(z, non_blocking=True)
             gp.step()
             out = gp.plan.out.clone()
@@ -307,19 +378,69 @@ class CompiledVAEDecoder:
         except Exception:  # noqa: BLE001
             return DecoderOutput(sample=out)
 
+    def encode(self, x, return_dict=True):
+        from .vae_plan import VAEEncodePlan
+        m = self._module
+        if x.dtype not in (torch.float16, torch.bfloat16):
+            self._warn_once("encode_dtype", "sfast (H100 build): VAE encode in %s is left on the module's eager "
+                            "path (the native encoder computes in fp16 / bf16)", x.dtype)
+            return self._eager_encode(x, return_dict=return_dict)
+        tile = getattr(m, "tile_sample_min_size", None)
+        if getattr(m, "use_tiling", False) and tile is not None and (x.shape[-1] > tile or x.shape[-2] > tile):
+            # diffusers' tiled encode blends overlapping tiles: different numbers from a whole-image encode
+            self._warn_once("encode_tiling", "sfast (H100 build): tiled VAE encode (use_tiling, image larger "
+                            "than %s) is left on the module's eager path", tile)
+            return self._eager_encode(x, return_dict=return_dict)
+        require_sm90(x.device)
+        with self._lock, torch.cuda.device(x.device):
+            gp = self._graphed("encode", VAEEncodePlan, x)
+            gp.plan.x_in.copy_(x, non_blocking=True)
+            gp.step()
+            moments = gp.plan.out.clone()
+        out_cls, dist_cls = _latent_dist_classes()
+        dist = dist_cls(moments)
+        if not return_dict:
+            return (dist,)
+        return out_cls(latent_dist=dist)
+
 
 def compile_vae_module(m, enable_cuda_graph=True):
-    """Replace ``m.decode`` of an AutoencoderKL (same module object; `encode` is left alone)."""
-    eager = m.decode
-    compiled = CompiledVAEDecoder(m.config, m.state_dict, eager, enable_cuda_graph)
+    """Replace ``m.decode`` and ``m.encode`` of an AutoencoderKL (same module object).  `encode` is
+    replaced only where the module has one and its encoder is supported; `decode` is kept where the VAE's
+    decoder is not the 2-D one (SVD's temporal decoder).  Either entry left alone is logged once."""
+    from .vae_plan import vae_encoder_spec_from_config
+    eager_decode = m.decode
+    if temporal_decoder(m.state_dict()):
+        logger.warning("sfast (H100 build): %s has no post_quant_conv (e.g. SVD's temporal decoder): its "
+                       "decode is left on the module's eager path", type(m).__name__)
+        eager_decode = None
+    eager_encode = getattr(m, "encode", None)
+    if eager_encode is not None:
+        try:
+            vae_encoder_spec_from_config(m.config)
+        except NotImplementedError as exc:
+            logger.warning("sfast (H100 build): VAE encode is left on the module's eager path (%s)", exc)
+            eager_encode = None
+    if eager_decode is None and eager_encode is None:
+        return m
+    compiled = CompiledVAE(m, eager_decode, eager_encode, enable_cuda_graph)
 
-    def decode(z, return_dict=True, generator=None):
-        return compiled(z, return_dict=return_dict, generator=generator)
+    if eager_decode is not None:
+        def decode(z, return_dict=True, generator=None):
+            return compiled.decode(z, return_dict=return_dict, generator=generator)
 
-    decode.__self__ = m
-    decode._cached = compiled._cached
-    decode._compiled = compiled
-    m.decode = decode
+        decode.__self__ = m
+        decode._cached = compiled._cached
+        decode._compiled = compiled
+        m.decode = decode
+    if eager_encode is not None:
+        def encode(x, return_dict=True):
+            return compiled.encode(x, return_dict=return_dict)
+
+        encode.__self__ = m
+        encode._cached = compiled._cached
+        encode._compiled = compiled
+        m.encode = encode
     return m
 
 

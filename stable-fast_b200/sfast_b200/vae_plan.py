@@ -1,5 +1,7 @@
-"""Launch schedule of the VAE decoder (diffusers ``AutoencoderKL.decode``), the module the reference's
-`compile_vae` wraps (/root/reference/src/sfast/compilers/diffusion_pipeline_compiler.py:154-190).
+"""Launch schedules of the VAE decoder and encoder (diffusers ``AutoencoderKL.decode`` / ``encode``), the
+module the reference's `compile_vae` wraps (/root/reference/src/sfast/compilers/diffusion_pipeline_compiler.py:
+154-190).  The encoder mirrors the decoder: GroupNorm-folded resnets, the same single-head attention, and
+stride-2 down-convs with diffusers' one-sided padding (SFB_A_DOWNCONV3X3) where the decoder has up-convs.
 
 Same kernel families as the UNet at larger spatial sizes: GroupNorm(+SiLU) -> implicit-GEMM 3x3
 convolutions with fused bias / residual, nearest-2x upsample folded into four 2x2 phase convolutions,
@@ -31,6 +33,7 @@ class VAESpec:
     groups: int
     eps: float = 1e-6
     num_frames: int = 0
+    in_channels: int = 3
 
     @property
     def temporal(self):
@@ -54,7 +57,22 @@ def vae_spec_from_config(cfg) -> VAESpec:
         raise NotImplementedError("VAE channel counts must be multiples of 64")
     return VAESpec(latent_channels=cfg_get(cfg, "latent_channels", 4), out_channels=cfg_get(cfg, "out_channels", 3),
                    block_out_channels=boc, layers_per_block=cfg_get(cfg, "layers_per_block", 2),
-                   groups=cfg_get(cfg, "norm_num_groups", 32))
+                   groups=cfg_get(cfg, "norm_num_groups", 32), in_channels=cfg_get(cfg, "in_channels", 3))
+
+
+def vae_encoder_spec_from_config(cfg) -> VAESpec:
+    """vae_spec_from_config plus what the native encoder needs of `AutoencoderKL.encode`."""
+    spec = vae_spec_from_config(cfg)
+    for t in cfg_get(cfg, "down_block_types", ("DownEncoderBlock2D",) * len(spec.block_out_channels)):
+        if t != "DownEncoderBlock2D":
+            raise NotImplementedError(f"VAE down block type {t}")
+    if not cfg_get(cfg, "double_z", True):
+        raise NotImplementedError("VAE config double_z=False is not supported by the H100 path")
+    if spec.in_channels > 8 or 2 * spec.latent_channels > 8:
+        # sfb_conv_in / sfb_conv_out take at most 8 image channels / moments
+        raise NotImplementedError(f"VAE encoder with {spec.in_channels} image channels and "
+                                  f"{2 * spec.latent_channels} moments (at most 8 each)")
+    return spec
 
 
 def vae_decoder_param_shapes(spec: VAESpec):
@@ -103,10 +121,54 @@ def vae_decoder_param_shapes(spec: VAESpec):
     return out
 
 
-class VAEDecodePlan(UNetPlan):
-    """Static launch schedule of `AutoencoderKL.decode` for a fixed (batch, latent height, width)."""
+def vae_encoder_param_shapes(spec: VAESpec):
+    """{diffusers parameter name: shape} of encoder + quant_conv."""
+    out = {}
 
-    def __init__(self, weights, batch, height, width):  # noqa: super().__init__ is UNet-specific
+    def conv(p, cout, cin, k):
+        out[p + ".weight"] = (cout, cin, k, k)
+        out[p + ".bias"] = (cout,)
+
+    def norm(p, c):
+        out[p + ".weight"] = (c,)
+        out[p + ".bias"] = (c,)
+
+    def resnet(p, cin, cout):
+        norm(p + ".norm1", cin)
+        conv(p + ".conv1", cout, cin, 3)
+        norm(p + ".norm2", cout)
+        conv(p + ".conv2", cout, cout, 3)
+        if cin != cout:
+            conv(p + ".conv_shortcut", cout, cin, 1)
+
+    boc, m = spec.block_out_channels, 2 * spec.latent_channels
+    conv("encoder.conv_in", boc[0], spec.in_channels, 3)
+    cout = boc[0]
+    for i, ch in enumerate(boc):
+        cin, cout = cout, ch
+        for j in range(spec.layers_per_block):
+            resnet(f"encoder.down_blocks.{i}.resnets.{j}", cin if j == 0 else cout, cout)
+        if i != len(boc) - 1:
+            conv(f"encoder.down_blocks.{i}.downsamplers.0.conv", cout, cout, 3)
+    c = boc[-1]
+    resnet("encoder.mid_block.resnets.0", c, c)
+    a = "encoder.mid_block.attentions.0"
+    norm(a + ".group_norm", c)
+    for n in ("to_q", "to_k", "to_v", "to_out.0"):
+        out[f"{a}.{n}.weight"] = (c, c)
+        out[f"{a}.{n}.bias"] = (c,)
+    resnet("encoder.mid_block.resnets.1", c, c)
+    norm("encoder.conv_norm_out", c)
+    conv("encoder.conv_out", m, c, 3)
+    conv("quant_conv", m, m, 1)
+    return out
+
+
+class _VAEPlan(UNetPlan):
+    """What the VAE's decoder and encoder schedules share: plan state without a time embedding or folded
+    LayerNorms, and the GroupNorm-folded resnet and single-head attention sub-graphs."""
+
+    def _init_vae(self, weights, batch, height, width, n_gn):  # noqa: UNetPlan.__init__ is UNet-specific
         self.controlnet, self.ctrl_in = False, []
         self.w, self.spec = weights, weights.spec
         self.dt, self.dev, self.dry = weights.dtype, weights.device, weights.dry
@@ -115,16 +177,10 @@ class VAEDecodePlan(UNetPlan):
         self.ops, self.side_ops = [], []
         self._side_stream, self._pending, self._gn_ws_patches, self._joined = None, None, [], True
         self._bufs, self._gn_count = {}, 0
-        spec = self.spec
-        self.z_in = self._alloc((batch, spec.latent_channels, height, width), self.dt)
-        up = 1 << (len(spec.block_out_channels) - 1)
-        self.out = self._alloc((batch, spec.out_channels, height * up, width * up), self.dt)
-        n_gn = 2 * (2 + len(spec.block_out_channels) * (spec.layers_per_block + 1)) + 2
         self._alloc_gn(n_gn, batch)
         self.ln_arena = self._alloc((2,), torch.float32)
         self._ln_used, self._ln_slots = 0, []
         self.ws, self._ws_need = None, 0
-        self._build()
 
     def vae_resnet(self, p, x: Act, dst: Act, cin, cout):
         eps = self.spec.eps
@@ -176,6 +232,19 @@ class VAEDecodePlan(UNetPlan):
         self.linear(p + ".to_out", o, self.w.matrix(p + ".to_out.0.weight"), self.w.f32(p + ".to_out.0.bias"),
                     dst, residual=x)
 
+
+class VAEDecodePlan(_VAEPlan):
+    """Static launch schedule of `AutoencoderKL.decode` for a fixed (batch, latent height, width)."""
+
+    def __init__(self, weights, batch, height, width):
+        spec = weights.spec
+        n_gn = 2 * (2 + len(spec.block_out_channels) * (spec.layers_per_block + 1)) + 2
+        self._init_vae(weights, batch, height, width, n_gn)
+        self.z_in = self._alloc((batch, spec.latent_channels, height, width), self.dt)
+        up = 1 << (len(spec.block_out_channels) - 1)
+        self.out = self._alloc((batch, spec.out_channels, height * up, width * up), self.dt)
+        self._build()
+
     def _build(self):
         spec, B, H, W, lib = self.spec, self.B, self.H, self.W, self.lib_or_dry()
         self._ws_token = _WsToken()
@@ -217,6 +286,67 @@ class VAEDecodePlan(UNetPlan):
                       (y.ptr, _ptr(w_out), _ptr(self.w.f32("decoder.conv_out.bias")), _ptr(self.out), B, h, w,
                        boc[0], spec.out_channels, y.ld, ops.dtype_code(self.dt)), (y.buf, w_out, self.out),
                       2 * B * h * w * boc[0] * 9 * spec.out_channels))
+        assert self._gn_count <= self.gn_stats.shape[0], (self._gn_count, self.gn_stats.shape)
+        if self._pending is not None:
+            self._pending["p"].defer_finish = 0
+            self._pending = None
+        self._ws_token.finalize(self)
+
+
+class VAEEncodePlan(_VAEPlan):
+    """Static launch schedule of `AutoencoderKL.encode` for a fixed (batch, image height, width): NCHW image
+    [B, in_channels, H, W] -> NCHW moments [B, 2 * latent_channels, H / 8, W / 8] (mean | logvar) of the
+    latent distribution.  quant_conv is folded into conv_out at pack time."""
+
+    def __init__(self, weights, batch, height, width):
+        spec = weights.spec
+        div = 1 << (len(spec.block_out_channels) - 1)
+        if height % div or width % div or (height // div) * (width // div) % 64:
+            # the mid-block attention runs P V with the token count as its K: a multiple of 64 (as in decode)
+            raise NotImplementedError(
+                f"sfast (H100 build): VAE encode of a {height}x{width} image: the size must be a multiple of "
+                f"{div} with a latent of a multiple of 64 pixels")
+        self._init_vae(weights, batch, height, width, 2 * (2 + len(spec.block_out_channels) * spec.layers_per_block) + 2)
+        self.x_in = self._alloc((batch, spec.in_channels, height, width), self.dt)
+        self.out = self._alloc((batch, 2 * spec.latent_channels, height // div, width // div), self.dt)
+        self._build()
+
+    def _build(self):
+        spec, B, H, W, lib = self.spec, self.B, self.H, self.W, self.lib_or_dry()
+        self._ws_token = _WsToken()
+        self._emit(Op("gn_sync.zero", lib.sfb_memset, (_ptr(self.gn_sync), 0, self.gn_sync.numel() * 4),
+                      (self.gn_sync,)))
+        boc, cin_img, m = spec.block_out_channels, spec.in_channels, 2 * spec.latent_channels
+        # conv_in (NCHW -> NHWC)
+        x = self.act("enc_x0", B, H, W, boc[0])
+        w_in = self.w.conv_in_weight("encoder.conv_in.weight")
+        self._emit(Op("encoder.conv_in", lib.sfb_conv_in,
+                      (_ptr(self.x_in), _ptr(w_in), _ptr(self.w.f32("encoder.conv_in.bias")), x.ptr, B, H, W, cin_img,
+                       boc[0], x.ld, ops.dtype_code(self.dt)), (self.x_in, w_in, x.buf), 2 * B * H * W * boc[0] * 9 * cin_img))
+        cout, h, w = boc[0], H, W
+        for i, ch in enumerate(boc):
+            cin, cout = cout, ch
+            for j in range(spec.layers_per_block):
+                dst = self.act(f"enc_down{i}_{j % 2}", B, h, w, cout)
+                self.vae_resnet(f"encoder.down_blocks.{i}.resnets.{j}", x, dst, cin if j == 0 else cout, cout)
+                x = dst
+            if i != len(boc) - 1:
+                dst = self.act(f"enc_ds{i}", B, h // 2, w // 2, cout)
+                name = f"encoder.down_blocks.{i}.downsamplers.0.conv"
+                self.conv3x3(name, x, name, dst, down=True)
+                x, h, w = dst, h // 2, w // 2
+        mid = "encoder.mid_block"
+        a = self.act("enc_mid0", B, h, w, cout)
+        b = self.act("enc_mid1", B, h, w, cout)
+        self.vae_resnet(mid + ".resnets.0", x, a, cout, cout)
+        self.vae_attention(mid + ".attentions.0", a, b)
+        self.vae_resnet(mid + ".resnets.1", b, a, cout, cout)
+        y = self.group_norm("encoder.conv_norm_out", a, "encoder.conv_norm_out", True, spec.eps)
+        # conv_out then quant_conv (1x1) as ONE 3x3 conv with the folded weight (NHWC -> NCHW)
+        w_out, b_out = self.w.conv3x3_pointwise("encoder.conv_out", "quant_conv")
+        self._emit(Op("encoder.conv_out+quant_conv", lib.sfb_conv_out,
+                      (y.ptr, _ptr(w_out), _ptr(b_out), _ptr(self.out), B, h, w, cout, m, y.ld, ops.dtype_code(self.dt)),
+                      (y.buf, w_out, b_out, self.out), 2 * B * h * w * m * (9 * cout + m)))
         assert self._gn_count <= self.gn_stats.shape[0], (self._gn_count, self.gn_stats.shape)
         if self._pending is not None:
             self._pending["p"].defer_finish = 0

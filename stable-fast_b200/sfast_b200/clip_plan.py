@@ -22,7 +22,7 @@ import torch
 
 from . import _lib, ops
 from .ops import Act, EPI_QKV, Op, _ptr
-from .plan import UNetPlan, _WsToken, _round_up
+from .plan import Plan, _round_up
 from .unet_spec import cfg_get
 
 _ACTS = {"quick_gelu": _lib.ACT_QUICK_GELU, "gelu": _lib.ACT_GELU}
@@ -40,7 +40,6 @@ class ClipTextSpec:
     eps: float
     eos_token_id: int
     projection_dim: int = 0  # > 0: CLIPTextModelWithProjection (text_projection, no bias)
-    groups: int = 32         # (unused: lets the UNet plan's helpers be shared)
 
     @property
     def temporal(self):
@@ -105,76 +104,47 @@ def random_clip_state_dict(spec: ClipTextSpec, dtype, device, seed=0):
     return sd
 
 
-class ClipTextPlan(UNetPlan):
-    """Static launch schedule of one text-encoder forward for a fixed (batch, sequence length)."""
+class _ClipPlan(Plan):
+    """What the text and vision towers share: [B, S] token rows, the encoder layers, and every layer's output
+    in its own buffer (hidden_states())."""
 
-    def __init__(self, weights, batch, seq):  # noqa: super().__init__ is UNet-specific
-        self.controlnet, self.ctrl_in = False, []
-        self.w, self.spec = weights, weights.spec
-        self.dt, self.dev, self.dry = weights.dtype, weights.device, weights.dry
-        self.lib = None if self.dry else _lib.lib()
-        self.B, self.S, self.H, self.W, self.ctx_len = batch, seq, 1, seq, 0
-        if seq > self.spec.max_positions:
-            raise ValueError(f"sequence length {seq} exceeds max_position_embeddings {self.spec.max_positions}")
-        self.ops, self.side_ops = [], []
-        self._side_stream, self._pending, self._gn_ws_patches, self._joined = None, None, [], True
-        self._bufs, self._gn_count = {}, 0
-        spec, rows = self.spec, batch * seq
-        self.ids_in = self._alloc((batch, seq), torch.int64)
-        self.gn_stats = self._alloc((1, 4), torch.float32)
-        self.gn_sync = self._alloc((1, 4), torch.int32)
-        # row statistics of every folded LayerNorm: 2 per layer + the embedding's
-        self.ln_arena = self._alloc(((2 * spec.layers + 1) * rows * 2 * ops.rowstats_slots(spec.hidden),), torch.float32)
-        self._ln_used, self._ln_slots = 0, []
-        self.ws, self._ws_need = None, 0
+    def __init__(self, weights, batch, seq, ln_floats):
+        super().__init__(weights, batch, 1, seq, ln_floats=ln_floats)
+        self.S = seq
         self.hidden = []       # [layers + 1] activations: embedding output, then every layer's output
         self.last_hidden_state = None
         self.pooled = None
-        self.text_embeds = None
-        self._build()
-        assert self._ln_used <= self.ln_arena.numel()
 
-    def _build(self):
-        spec, B, S, lib = self.spec, self.B, self.S, self.lib_or_dry()
-        C, H, D, I = spec.hidden, spec.heads, spec.head_dim, spec.intermediate
-        rows = B * S
-        self._ws_token = _WsToken()
-        self._emit(Op("ln_stats.zero", lib.sfb_memset, (_ptr(self.ln_arena), 0, self.ln_arena.numel() * 4),
-                      (self.ln_arena,)))
-        hs = self.act("clip_h0", B, 1, S, C)
-        st = self._ln_view(self.ln_slot(rows, C))
-        tok = self.w.small("text_model.embeddings.token_embedding.weight")
-        pos = self.w.small("text_model.embeddings.position_embedding.weight")
-        self._emit(Op("embeddings", lib.sfb_embed_tokens,
-                      (_ptr(self.ids_in), _ptr(tok), _ptr(pos), hs.ptr, _ptr(st), st.slots, B, S, C, spec.vocab_size, hs.ld,
-                       ops.dtype_code(self.dt)), (self.ids_in, tok, pos, hs.buf, st), 0, 4 * rows * C))
-        self.hidden.append(hs)
-        dv = _round_up(D + 1, 16)
-        q_pitch, vt_pitch = _round_up(D, 64), _round_up(S, 64)
-        q = self.buf("clip_q", (B * H * S, q_pitch))
-        k = self.buf("clip_k", (B * H * S, q_pitch))
-        vt = self.buf("clip_vt", (B * H * dv, vt_pitch))
-        if not self.dry:
-            vt.view(B * H, dv, vt_pitch)[:, D, :] = 1.0  # the ones row: softmax denominators on the tensor core
-        qkv = dict(q=q, k=k, vt=vt, heads=H, head_dim=D, q_pitch=q_pitch, q_rows=S, k_rows=S, vt_rows=dv,
-                   vt_pitch=vt_pitch, which_base=0, seq=S)
+    def encoder(self, prefix, hs: Act, st, **attn):
+        """The encoder layers of `prefix` ("text_model" / "vision_model") on hs; returns the last layer's output.
+        Per layer: LayerNorm1 folded into the fused QKV projection -> attention (`attn`: attention_op options)
+        -> out_proj + residual -> LayerNorm2 folded into fc1 + activation -> fc2 + residual.  `st`: hs's row
+        statistics; None where no GEMM epilogue produced them (the vision tower's pre-LayerNorm output), and
+        then layer 0's LayerNorm1 is the stand-alone kernel."""
+        spec, B, S = self.spec, self.B, self.S
+        C, I, rows = spec.hidden, spec.intermediate, B * S
+        qkv = self.attention_operands(B, spec.heads, S, S, spec.head_dim)
+        qkv_epi = dict(qkv, which_base=0, seq=S)
         for l in range(spec.layers):
-            p = f"text_model.encoder.layers.{l}"
+            p = f"{prefix}.encoder.layers.{l}"
             a = p + ".self_attn"
-            wm, bias, colsum = self.w.ln_matrix(
-                [f"{a}.q_proj.weight", f"{a}.k_proj.weight", f"{a}.v_proj.weight"], p + ".layer_norm1",
-                bias_names=[f"{a}.q_proj.bias", f"{a}.k_proj.bias", f"{a}.v_proj.bias"])
-            self._emit(self._gemm(a + ".qkv", a=self._a_matrix(hs), b=wm, M=rows, N=wm.n, K=C, dt=self.dt,
-                                  epi=EPI_QKV, bias=bias, qkv=qkv, splits=1,
-                                  ln=dict(rowstats=st, colsum=colsum, eps=spec.eps, dim=C),
-                                  keep=(hs.buf, wm, colsum)))
+            wn = [f"{a}.{n}_proj.weight" for n in "qkv"]
+            bn = [f"{a}.{n}_proj.bias" for n in "qkv"]
+            if st is None:
+                x1 = self.layer_norm(p + ".layer_norm1", hs, p + ".layer_norm1", spec.eps)
+                wm = self.w.cat_matrix(wn)
+                self._emit(self._gemm(a + ".qkv", a=self._a_matrix(x1), b=wm, M=rows, N=wm.n, K=C, dt=self.dt,
+                                      epi=EPI_QKV, bias=self.w.f32_cat(bn), qkv=qkv_epi, splits=1, keep=(x1.buf, wm)))
+            else:
+                wm, bias, colsum = self.w.ln_matrix(wn, p + ".layer_norm1", bias_names=bn)
+                self._emit(self._gemm(a + ".qkv", a=self._a_matrix(hs), b=wm, M=rows, N=wm.n, K=C, dt=self.dt,
+                                      epi=EPI_QKV, bias=bias, qkv=qkv_epi, splits=1,
+                                      ln=dict(rowstats=st, colsum=colsum, eps=spec.eps, dim=C),
+                                      keep=(hs.buf, wm, colsum)))
             ao = self.act("clip_attn_out", B, 1, S, C)
-            self._emit(ops.attention_op(a + ".core", lib, q=q, k=k, vt=vt, out=ao.buf, batch=B, heads=H,
-                                        head_dim=D, seq_q=S, seq_kv=S, q_rows=S, k_rows=S, vt_rows=dv,
-                                        q_pitch=q_pitch, vt_pitch=vt_pitch, dt=self.dt, dry=self.dry, kv_tile=64,
-                                        causal=True))
+            self.attention_core(a + ".core", qkv, ao, **attn)
             mid = self.act("clip_mid", B, 1, S, C)
-            st2 = self._ln_view(self.ln_slot(rows, C))
+            st2 = self.ln_slot(rows, C)
             self.linear(a + ".out_proj", ao, self.w.matrix(f"{a}.out_proj.weight"), self.w.f32(f"{a}.out_proj.bias"),
                         mid, residual=hs, rowstats_out=st2, splits=1)
             w1, b1, cs1 = self.w.ln_matrix([p + ".mlp.fc1.weight"], p + ".layer_norm2",
@@ -185,15 +155,45 @@ class ClipTextPlan(UNetPlan):
                                   ln=dict(rowstats=st2, colsum=cs1, eps=spec.eps, dim=C),
                                   keep=(mid.buf, ff.buf, w1, cs1)))
             nxt = self.act(f"clip_h{l + 1}", B, 1, S, C)
-            st = self._ln_view(self.ln_slot(rows, C)) if l + 1 < spec.layers else None
+            st = self.ln_slot(rows, C) if l + 1 < spec.layers else None
             self.linear(p + ".mlp.fc2", ff, self.w.matrix(p + ".mlp.fc2.weight"), self.w.f32(p + ".mlp.fc2.bias"),
                         nxt, residual=mid, rowstats_out=st, splits=1)
             hs = nxt
             self.hidden.append(hs)
-        out = self.act("clip_last", B, 1, S, C)
-        self._emit(ops.ln_op("final_layer_norm", lib, x=hs.buf, y=out.buf, rows=rows, c=C,
-                             gamma=self.w.f32("text_model.final_layer_norm.weight"),
-                             beta=self.w.f32("text_model.final_layer_norm.bias"), eps=spec.eps, dt=self.dt))
+        return hs
+
+    def hidden_states(self):
+        """Tuple of [B, S, C] views: embedding output, then each encoder layer's output."""
+        return tuple(h.buf.view(self.B, self.S, self.spec.hidden) for h in self.hidden)
+
+
+class ClipTextPlan(_ClipPlan):
+    """Static launch schedule of one text-encoder forward for a fixed (batch, sequence length)."""
+
+    def __init__(self, weights, batch, seq):
+        spec = weights.spec
+        if seq > spec.max_positions:
+            raise ValueError(f"sequence length {seq} exceeds max_position_embeddings {spec.max_positions}")
+        # row statistics of every folded LayerNorm: 2 per layer + the embedding's
+        super().__init__(weights, batch, seq,
+                         (2 * spec.layers + 1) * batch * seq * 2 * ops.rowstats_slots(spec.hidden))
+        self.ids_in = self._alloc((batch, seq), torch.int64)
+        self.text_embeds = None
+        self._build()
+
+    def _build(self):
+        spec, B, S, lib = self.spec, self.B, self.S, self.lib_or_dry()
+        C, rows = spec.hidden, B * S
+        hs = self.act("clip_h0", B, 1, S, C)
+        st = self.ln_slot(rows, C)
+        tok = self.w.small("text_model.embeddings.token_embedding.weight")
+        pos = self.w.small("text_model.embeddings.position_embedding.weight")
+        self._emit(Op("embeddings", lib.sfb_embed_tokens,
+                      (_ptr(self.ids_in), _ptr(tok), _ptr(pos), hs.ptr, _ptr(st), st.slots, B, S, C, spec.vocab_size, hs.ld,
+                       ops.dtype_code(self.dt)), (self.ids_in, tok, pos, hs.buf, st), 0, 4 * rows * C))
+        self.hidden.append(hs)
+        hs = self.encoder("text_model", hs, st, kv_tile=64, causal=True)
+        out = self.layer_norm("final_layer_norm", hs, "text_model.final_layer_norm", spec.eps)
         self.last_hidden_state = out.buf.view(B, S, C) if not self.dry else out.buf
         self.pooled = self.buf("clip_pooled", (B, C))
         self._emit(Op("pool(eos)", lib.sfb_clip_pool,
@@ -204,11 +204,7 @@ class ClipTextPlan(UNetPlan):
             self._emit(ops.small_linear_op("text_projection", lib, x=self.pooled,
                                            w=self.w.small("text_projection.weight"), bias=None, batch=B,
                                            n=spec.projection_dim, k=C, dt=self.dt, y16=self.text_embeds))
-        self._ws_token.finalize(self)
-
-    def hidden_states(self):
-        """Tuple of [B, S, C] views: embedding output, then each encoder layer's output."""
-        return tuple(h.buf.view(self.B, self.S, self.spec.hidden) for h in self.hidden)
+        self._finish()
 
 
 # =================================================================================================
@@ -228,7 +224,6 @@ class ClipVisionSpec:
     act: str
     eps: float
     projection_dim: int = 0  # > 0: CLIPVisionModelWithProjection (visual_projection, no bias)
-    groups: int = 32
 
     @property
     def temporal(self):
@@ -290,72 +285,21 @@ def clip_vision_param_shapes(spec: ClipVisionSpec):
     return out
 
 
-class ClipVisionPlan(UNetPlan):
+class ClipVisionPlan(_ClipPlan):
     """Static launch schedule of one vision-tower forward for a fixed batch of image_size^2 images."""
 
-    def __init__(self, weights, batch):  # noqa: super().__init__ is UNet-specific
-        self.controlnet, self.ctrl_in = False, []
-        self.w, self.spec = weights, weights.spec
-        self.dt, self.dev, self.dry = weights.dtype, weights.device, weights.dry
-        self.lib = None if self.dry else _lib.lib()
-        spec = self.spec
-        self.B, self.S, self.H, self.W, self.ctx_len = batch, spec.tokens, 1, spec.tokens, 0
-        self.ops, self.side_ops = [], []
-        self._side_stream, self._pending, self._gn_ws_patches, self._joined = None, None, [], True
-        self._bufs, self._gn_count = {}, 0
-        rows = batch * spec.tokens
+    def __init__(self, weights, batch):
+        spec = weights.spec
+        super().__init__(weights, batch, spec.tokens,
+                         2 * spec.layers * batch * spec.tokens * 2 * ops.rowstats_slots(spec.hidden))
         self.pixels_in = self._alloc((batch, spec.channels, spec.image_size, spec.image_size), self.dt)
-        self.gn_stats = self._alloc((1, 4), torch.float32)
-        self.gn_sync = self._alloc((1, 4), torch.int32)
-        self.ln_arena = self._alloc((2 * spec.layers * rows * 2 * ops.rowstats_slots(spec.hidden),), torch.float32)
-        self._ln_used, self._ln_slots = 0, []
-        self.ws, self._ws_need = None, 0
-        self.hidden = []
-        self.pooled = self.image_embeds = None
+        self.image_embeds = None
         self._build()
-        assert self._ln_used <= self.ln_arena.numel()
-
-    # ---- weights the vision tower needs in forms the UNet never does (registered for refresh())
-    def _patch_matrix(self, kpad):
-        name = "vision_model.embeddings.patch_embedding.weight"
-
-        def build():
-            w = self.w._raw(name).to(self.w.device)
-            w2 = w.reshape(w.shape[0], -1)
-            if w2.device.type == "meta":
-                wp = torch.empty(w2.shape[0], kpad, dtype=self.dt, device="meta")
-            else:
-                wp = torch.zeros(w2.shape[0], kpad, dtype=self.dt, device=w2.device)
-                wp[:, :w2.shape[1]] = w2.to(self.dt)
-            return self.w._mat(wp)
-        return self.w._get(("patch_mat", kpad), build)
-
-    def _cls_row(self):
-        def build():
-            e = "vision_model.embeddings"
-            v = self.w._raw(e + ".class_embedding").to(self.w.device).float() + \
-                self.w._raw(e + ".position_embedding.weight").to(self.w.device)[0].float()
-            return v.to(self.dt).reshape(1, -1).contiguous()
-        return self.w._get(("cls_row",), build)
-
-    def _pos_rest(self):
-        def build():
-            return self.w._raw("vision_model.embeddings.position_embedding.weight").to(
-                device=self.w.device, dtype=self.dt)[1:].contiguous()
-        return self.w._get(("pos_rest",), build)
-
-    def _f32_cat(self, names):
-        return self.w._get(("f32cat",) + tuple(names), lambda: torch.cat(
-            [self.w._raw(n).to(device=self.w.device, dtype=torch.float32) for n in names]).contiguous())
 
     def _build(self):
         spec, B, S, lib = self.spec, self.B, self.S, self.lib_or_dry()
-        C, H, D, I = spec.hidden, spec.heads, spec.head_dim, spec.intermediate
-        rows, np_ = B * S, spec.grid * spec.grid
+        C, rows, np_ = spec.hidden, B * S, spec.grid * spec.grid
         es = 2
-        self._ws_token = _WsToken()
-        self._emit(Op("ln_stats.zero", lib.sfb_memset, (_ptr(self.ln_arena), 0, self.ln_arena.numel() * 4),
-                      (self.ln_arena,)))
         # ---- embeddings: patchify -> GEMM (+ position embedding as the residual) per image; class rows copied
         kreal = spec.channels * spec.patch_size ** 2
         kpad = _round_up(kreal, 64)
@@ -364,7 +308,10 @@ class ClipVisionPlan(UNetPlan):
                       (_ptr(self.pixels_in), _ptr(patches), B, spec.channels, spec.image_size, spec.image_size,
                        spec.patch_size, kpad), (self.pixels_in, patches), 0, 4 * B * np_ * kpad))
         emb = self.act("clipv_emb", B, 1, S, C)
-        wm, pos, cls = self._patch_matrix(kpad), self._pos_rest(), self._cls_row()
+        e = "vision_model.embeddings"
+        wm = self.w.patch_matrix(e + ".patch_embedding.weight", kpad)
+        pos = self.w.rows_from_1(e + ".position_embedding.weight")
+        cls = self.w.class_row(e + ".class_embedding", e + ".position_embedding.weight")
         for b in range(B):
             dst = emb.ptr + (b * S + 1) * C * es
             self._emit(self._gemm(f"patch_embedding[{b}]", a=ops.a_matrix(_ptr(patches) + b * np_ * kpad * es, np_, kpad, kpad),
@@ -372,63 +319,12 @@ class ClipVisionPlan(UNetPlan):
                                   splits=1, keep=(patches, emb.buf, wm, pos)))
             self._emit(Op(f"class_embedding[{b}]", lib.sfb_copy2d, (_ptr(cls), emb.ptr + b * S * C * es, 1, C, C, C),
                           (cls, emb.buf)))
-        hs = self.act("clipv_h0", B, 1, S, C)
+        hs = self.act("clip_h0", B, 1, S, C)
         self._emit(ops.ln_op("pre_layrnorm", lib, x=emb.buf, y=hs.buf, rows=rows, c=C,
                              gamma=self.w.f32("vision_model.pre_layrnorm.weight"),
                              beta=self.w.f32("vision_model.pre_layrnorm.bias"), eps=spec.eps, dt=self.dt))
         self.hidden.append(hs)
-        dv = _round_up(D + 1, 16)
-        q_pitch, vt_pitch = _round_up(D, 64), _round_up(S, 64)
-        q = self.buf("clipv_q", (B * H * S, q_pitch))
-        k = self.buf("clipv_k", (B * H * S, q_pitch))
-        vt = self.buf("clipv_vt", (B * H * dv, vt_pitch))
-        if not self.dry:
-            vt.view(B * H, dv, vt_pitch)[:, D, :] = 1.0
-        qkv = dict(q=q, k=k, vt=vt, heads=H, head_dim=D, q_pitch=q_pitch, q_rows=S, k_rows=S, vt_rows=dv,
-                   vt_pitch=vt_pitch, which_base=0, seq=S)
-        st = None
-        for l in range(spec.layers):
-            p = f"vision_model.encoder.layers.{l}"
-            a = p + ".self_attn"
-            wn = [f"{a}.q_proj.weight", f"{a}.k_proj.weight", f"{a}.v_proj.weight"]
-            bn = [f"{a}.q_proj.bias", f"{a}.k_proj.bias", f"{a}.v_proj.bias"]
-            if st is None:
-                # layer 0 reads the pre-LayerNorm's output, whose row statistics no GEMM epilogue produced:
-                # its first LayerNorm is the stand-alone kernel
-                x1 = self.act("clipv_ln1", B, 1, S, C)
-                self._emit(ops.ln_op(p + ".layer_norm1", lib, x=hs.buf, y=x1.buf, rows=rows, c=C,
-                                     gamma=self.w.f32(p + ".layer_norm1.weight"),
-                                     beta=self.w.f32(p + ".layer_norm1.bias"), eps=spec.eps, dt=self.dt))
-                wm = self.w.cat_matrix(wn)
-                self._emit(self._gemm(a + ".qkv", a=self._a_matrix(x1), b=wm, M=rows, N=wm.n, K=C, dt=self.dt,
-                                      epi=EPI_QKV, bias=self._f32_cat(bn), qkv=qkv, splits=1, keep=(x1.buf, wm)))
-            else:
-                wm, bias, colsum = self.w.ln_matrix(wn, p + ".layer_norm1", bias_names=bn)
-                self._emit(self._gemm(a + ".qkv", a=self._a_matrix(hs), b=wm, M=rows, N=wm.n, K=C, dt=self.dt,
-                                      epi=EPI_QKV, bias=bias, qkv=qkv, splits=1,
-                                      ln=dict(rowstats=st, colsum=colsum, eps=spec.eps, dim=C),
-                                      keep=(hs.buf, wm, colsum)))
-            ao = self.act("clipv_attn_out", B, 1, S, C)
-            self._emit(ops.attention_op(a + ".core", lib, q=q, k=k, vt=vt, out=ao.buf, batch=B, heads=H,
-                                        head_dim=D, seq_q=S, seq_kv=S, q_rows=S, k_rows=S, vt_rows=dv,
-                                        q_pitch=q_pitch, vt_pitch=vt_pitch, dt=self.dt, dry=self.dry))
-            mid = self.act("clipv_mid", B, 1, S, C)
-            st2 = self._ln_view(self.ln_slot(rows, C))
-            self.linear(a + ".out_proj", ao, self.w.matrix(f"{a}.out_proj.weight"), self.w.f32(f"{a}.out_proj.bias"),
-                        mid, residual=hs, rowstats_out=st2, splits=1)
-            w1, b1, cs1 = self.w.ln_matrix([p + ".mlp.fc1.weight"], p + ".layer_norm2",
-                                           bias_names=[p + ".mlp.fc1.bias"])
-            ff = self.act("clipv_ff", B, 1, S, I)
-            self._emit(self._gemm(p + ".mlp.fc1", a=self._a_matrix(mid), b=w1, M=rows, N=I, K=C, dt=self.dt,
-                                  out=ff.ptr, ldo=ff.ld, bias=b1, splits=1, act=_ACTS[spec.act],
-                                  ln=dict(rowstats=st2, colsum=cs1, eps=spec.eps, dim=C),
-                                  keep=(mid.buf, ff.buf, w1, cs1)))
-            nxt = self.act(f"clipv_h{l + 1}", B, 1, S, C)
-            st = self._ln_view(self.ln_slot(rows, C)) if l + 1 < spec.layers else None
-            self.linear(p + ".mlp.fc2", ff, self.w.matrix(p + ".mlp.fc2.weight"), self.w.f32(p + ".mlp.fc2.bias"),
-                        nxt, residual=mid, rowstats_out=st, splits=1)
-            hs = nxt
-            self.hidden.append(hs)
+        hs = self.encoder("vision_model", hs, None)
         self.last_hidden_state = hs.buf.view(B, S, C) if not self.dry else hs.buf
         # pooled = post_layernorm(class-token rows); image_embeds = visual_projection(pooled)
         cls_rows = self.buf("clipv_cls", (B, C))
@@ -443,7 +339,4 @@ class ClipVisionPlan(UNetPlan):
             self._emit(ops.small_linear_op("visual_projection", lib, x=self.pooled,
                                            w=self.w.small("visual_projection.weight"), bias=None, batch=B,
                                            n=spec.projection_dim, k=C, dt=self.dt, y16=self.image_embeds))
-        self._ws_token.finalize(self)
-
-    def hidden_states(self):
-        return tuple(h.buf.view(self.B, self.S, self.spec.hidden) for h in self.hidden)
+        self._finish()

@@ -130,17 +130,43 @@ class PackedWeights:
             return ops.pack_conv3x3(w, self.dtype), b.float().contiguous()
         return self._get(("c3pw", conv, pointwise), build)
 
+    def _padded_mat(self, w, kpad):
+        """[n, k] weight zero-padded along K to kpad columns, as a GEMM operand."""
+        if w.device.type == "meta":
+            wp = torch.empty(w.shape[0], kpad, dtype=self.dtype, device="meta")
+        else:
+            wp = torch.zeros(w.shape[0], kpad, dtype=self.dtype, device=w.device)
+            wp[:, :w.shape[1]] = w.to(self.dtype)
+        return self._mat(wp)
+
     def conv_in_matrix(self, name):
         """First conv as a GEMM operand: [cout, (kh, kw, cin)] zero-padded along K to 64."""
+        return self._get(("cin_mat", name), lambda: self._padded_mat(
+            ops.pack_conv3x3(self._raw(name).to(self.device), self.dtype), 64))
+
+    def patch_matrix(self, name, kpad):
+        """Patch-embedding conv [cout, cin, p, p] as a GEMM operand over patchified rows: [cout, (cin, p, p)]
+        zero-padded along K to kpad."""
         def build():
-            w = ops.pack_conv3x3(self._raw(name).to(self.device), self.dtype)
-            if w.device.type == "meta":
-                wp = torch.empty(w.shape[0], 64, dtype=self.dtype, device="meta")
-            else:
-                wp = torch.zeros(w.shape[0], 64, dtype=self.dtype, device=w.device)
-                wp[:, :w.shape[1]] = w
-            return self._mat(wp)
-        return self._get(("cin_mat", name), build)
+            w = self._raw(name).to(self.device)
+            return self._padded_mat(w.reshape(w.shape[0], -1), kpad)
+        return self._get(("patch_mat", name, kpad), build)
+
+    def class_row(self, class_name, pos_name):
+        """[1, c] class embedding plus the first position embedding: the class token's input row."""
+        def build():
+            v = self._raw(class_name).to(self.device).float() + self._raw(pos_name).to(self.device)[0].float()
+            return v.to(self.dtype).reshape(1, -1).contiguous()
+        return self._get(("cls_row", class_name, pos_name), build)
+
+    def rows_from_1(self, name):
+        """Rows 1.. of a [n, c] table (the patch tokens' position embeddings)."""
+        return self._get(("rows1", name), lambda: self._raw(name).to(
+            device=self.device, dtype=self.dtype)[1:].contiguous())
+
+    def f32_cat(self, names):
+        return self._get(("f32cat",) + tuple(names), lambda: torch.cat(
+            [self._raw(n).to(device=self.device, dtype=torch.float32) for n in names]).contiguous())
 
     def conv_in_weight(self, name):
         return self._get(("cin", name), lambda: ops.pack_conv_in(self._raw(name).to(self.device),
@@ -220,26 +246,22 @@ class PackedWeights:
             device=self.device, dtype=self.dtype).contiguous())
 
 
-class UNetPlan:
-    """One static launch schedule for a fixed (batch, height, width)."""
+class Plan:
+    """One static launch schedule over pre-allocated buffers, for a fixed (batch, height, width): the state and
+    the emitters every model's schedule shares.  `n_gn`: GroupNorms the schedule runs (their statistics arenas
+    are allocated only when > 0); `ln_floats`: fp32 row statistics of its folded LayerNorms.  Both arenas
+    are zeroed at the start of every step; `_finish()` closes the schedule."""
 
-    def __init__(self, weights: PackedWeights, batch, height, width, ctx_len=77, controlnet=False):
-        self.controlnet = controlnet
-        self.ctrl_in = []  # static NCHW inputs: 12 (SD-1.5) down-block residuals + the mid-block one
+    def __init__(self, weights: PackedWeights, batch, height, width, *, n_gn=0, ln_floats=0):
         self.w = weights
         self.spec = weights.spec
         self.dt, self.dev, self.dry = weights.dtype, weights.device, weights.dry
         self.lib = None if self.dry else _lib.lib()
-        self.B, self.H, self.W, self.ctx_len = batch, height, width, ctx_len
-        div = 1 << (len(self.spec.block_out_channels) - 1)
-        if height % div or width % div:
-            # diffusers switches to explicit upsample sizes there (forward_upsample_size); not built
-            raise NotImplementedError(
-                f"sfast (H100 build): latent size {height}x{width} must be a multiple of {div}")
+        self.B, self.H, self.W = batch, height, width
         self.ops = []
-        # Ops that depend only on the step's inputs (cross-attention K/V projections of the text
-        # embedding): issued on a forked stream so they run concurrently with the start of the
-        # main chain (a parallel branch of the captured CUDA graph).
+        # Ops that depend only on the step's inputs (e.g. the UNet's cross-attention K/V projections of the
+        # text embedding): issued on a forked stream so they run concurrently with the start of the main
+        # chain (a parallel branch of the captured CUDA graph).
         self.side_ops = []
         self._side_stream = None
         self._pending = None      # conv GEMM whose split-K finish the next GroupNorm may absorb
@@ -247,65 +269,39 @@ class UNetPlan:
         self._joined = False
         self._bufs = {}
         self._gn_count = 0
-        spec = self.spec
-        nres = len(spec.down)
-        if height % (1 << (nres - 1)) or width % (1 << (nres - 1)):
-            raise NotImplementedError(f"latent {height}x{width} must be divisible by {1 << (nres - 1)}")
-        # ---- static inputs / output
-        self.sample_in = self._alloc((batch, spec.in_channels, height, width), self.dt)
-        self.t_in = self._alloc((batch,), torch.float32)
-        self.ehs_in = self._alloc((batch, ctx_len, spec.cross_attention_dim), self.dt)
-        self.out = self._alloc((batch, spec.out_channels, height, width), self.dt)
-        if spec.addition_embed_type == "text_time":
-            self.add_in = self._alloc((batch, spec.add_in_dim), self.dt)
-            self.time_ids_in = self._alloc((batch * 6,), torch.float32)
-        n_gn = sum(2 for _ in spec.all_resnets()) + 1
-        for blk in spec.down + [spec.mid] + spec.up:
-            n_gn += sum(1 for t in blk.attentions if t is not None)
-        self._alloc_gn(n_gn, batch)
-        # folded-LayerNorm row statistics: [rows, 2] fp32 per LayerNorm, zeroed once per step
+        self._n_gn = n_gn
+        lib = self.lib_or_dry()
+        if n_gn:
+            # per-GroupNorm statistics workspace (one [groups][2] slot per CTA of the statistics pass, summed in
+            # a fixed order by the apply pass: no initialisation needed) and the fused kernel's grid-barrier
+            # counters (zeroed once per step)
+            self.gn_stats = self._alloc((n_gn, ops.gn_ws_floats(batch, self.spec.groups)), torch.float32)
+            self.gn_sync = self._alloc((n_gn, 4), torch.int32)
+            # GroupNorm folded into the conv: per-image tickets of the statistics kernel (self-resetting)
+            self.gn_tickets = self._alloc((n_gn, max(batch, 4)), torch.int32)
+            self._emit(Op("gn_sync.zero", lib.sfb_memset, (_ptr(self.gn_sync), 0, self.gn_sync.numel() * 4),
+                          (self.gn_sync,)))
+        # folded-LayerNorm row statistics: [rows, slots, 2] fp32 per LayerNorm (ln_slot)
         self._ln_used = 0
-        self._ln_slots = []
-        self.ln_arena = self._alloc((max(self._ln_arena_floats(), 2),), torch.float32)
-        self.ws = None
-        self._ws_need = 0
-        self._build()
+        self.ln_arena = self._alloc((max(ln_floats, 2),), torch.float32)
+        if ln_floats:
+            self._emit(Op("ln_stats.zero", lib.sfb_memset, (_ptr(self.ln_arena), 0, self.ln_arena.numel() * 4),
+                          (self.ln_arena,)))
+        # split-K workspace: one shared fp32 buffer, sized by _finish() once all ops are known
+        self._ws_token = _WsToken()
+
+    def _finish(self):
+        """Close the schedule: a deferred split-K finish nothing consumed is done by its own GEMM; check the
+        GroupNorm and LayerNorm budgets; allocate the split-K workspace and patch the ops."""
+        if self._pending is not None:
+            self._pending["p"].defer_finish = 0
+            self._pending = None
+        assert self._gn_count == self._n_gn, (self._gn_count, self._n_gn)
         assert self._ln_used <= self.ln_arena.numel(), (self._ln_used, self.ln_arena.numel())
-
-    def _alloc_gn(self, n_gn, max_images):
-        """Per-GroupNorm statistics workspace (one [groups][2] slot per CTA of the statistics pass, summed
-        in a fixed order by the apply pass: no initialisation needed) and the fused kernel's grid-barrier
-        counters (zeroed once per step)."""
-        self.gn_stats = self._alloc((n_gn, ops.gn_ws_floats(max_images, self.spec.groups)), torch.float32)
-        self.gn_sync = self._alloc((n_gn, 4), torch.int32)
-        # GroupNorm folded into the conv: per-image tickets of the statistics kernel (self-resetting)
-        self.gn_tickets = self._alloc((n_gn, max(max_images, 4)), torch.int32)
-
-    def _ln_arena_floats(self):
-        """3 * depth LayerNorms per transformer, each [B*h*w, slots(dim), 2] floats at its resolution."""
-        spec, tot = self.spec, 0
-        h, w = self.H, self.W
-
-        def need(blk):
-            return sum(3 * t.depth * self.B * h * w * 2 * ops.rowstats_slots(t.dim)
-                       for t in blk.attentions if t is not None)
-        for blk in spec.down:
-            tot += need(blk)
-            if blk.sampler:
-                h, w = h // 2, w // 2
-        tot += need(spec.mid)
-        for blk in spec.up:
-            tot += need(blk)
-            if blk.sampler:
-                h, w = h * 2, w * 2
-        return tot
-
-    def _ln_view(self, slot):
-        _, off, rows, slots = slot
-        return ops.RowStats(self.ln_arena[off:off + rows * slots * 2], slots)
+        self._ws_token.finalize(self)
 
     # ------------------------------------------------------------------ buffers
-    def _alloc(self, shape, dtype, zero=True):
+    def _alloc(self, shape, dtype):
         if self.dry:
             return torch.empty(shape, dtype=dtype, device="meta")
         return torch.zeros(shape, dtype=dtype, device=self.dev)
@@ -319,9 +315,13 @@ class UNetPlan:
     def act(self, name, n, h, w, c):
         return Act(self.buf(name, (n, h, w, c)), n, h, w, c)
 
-    def activation_bytes(self):
-        tot = sum(b.numel() * b.element_size() for b in self._bufs.values())
-        return tot + self.gn_stats.numel() * 4
+    def ln_slot(self, rows, dim):
+        """[rows, slots, 2] fp32 (sum, sum of squares) statistics of one folded LayerNorm over `dim`
+        columns: every producer writes its own slots, the consumer adds them in order."""
+        slots = ops.rowstats_slots(dim)
+        off = self._ln_used
+        self._ln_used += rows * slots * 2
+        return ops.RowStats(self.ln_arena[off:off + rows * slots * 2], slots)
 
     # ------------------------------------------------------------------ op emitters
     def _emit(self, op):
@@ -336,7 +336,6 @@ class UNetPlan:
             self.ops.append(op)
 
     def _gemm(self, name, **kw):
-        # split-K workspace: one shared fp32 buffer, sized after all ops are known
         kw.setdefault("ws", self._ws_token)
         return ops.gemm_op(name, self.lib_or_dry(), dry=self.dry, **kw)
 
@@ -474,6 +473,146 @@ class UNetPlan:
         op = self._gemm(name, **kw)
         self._emit(op)
 
+    def layer_norm(self, name, x: Act, prefix, eps=1e-5):
+        y = self.act("ln_out", x.n, x.h, x.w, x.c)
+        self._emit(ops.ln_op(name, self.lib_or_dry(), x=x.buf, y=y.buf, rows=x.rows, c=x.c,
+                             gamma=self.w.f32(prefix + ".weight"), beta=self.w.f32(prefix + ".bias"),
+                             eps=eps, dt=self.dt))
+        return y
+
+    def attention_operands(self, B, H, S, skv, D, kv_tag=""):
+        """q [B*H*S, q_pitch], k [B*H*skv, q_pitch] and v^T [B*H*dv, vt_pitch] buffers of one flash-attention
+        launch, as the QKV-scatter epilogue and the attention kernel address them.  v^T carries an all-ones
+        row after the D value rows: P times it is the softmax denominator, computed on the tensor core.
+        `kv_tag` keeps k / v^T apart from other launches of the same shape (the UNet's hoisted cross K/V)."""
+        dv = _round_up(D + 1, 16)
+        q_pitch, vt_pitch = _round_up(D, 64), _round_up(skv, 64)
+        tag = f"{B}x{H}x{S}x{skv}x{D}"
+        q = self.buf("attn_q_" + tag, (B * H * S, q_pitch))
+        k = self.buf("attn_k_" + tag + kv_tag, (B * H * skv, q_pitch))
+        new_vt = ("attn_vt_" + tag + kv_tag, (B * H * dv, vt_pitch), self.dt) not in self._bufs
+        vt = self.buf("attn_vt_" + tag + kv_tag, (B * H * dv, vt_pitch))
+        if new_vt and not self.dry:
+            vt.view(B * H, dv, vt_pitch)[:, D, :] = 1.0
+        return dict(q=q, k=k, vt=vt, heads=H, head_dim=D, q_pitch=q_pitch, q_rows=S, k_rows=skv,
+                    vt_rows=dv, vt_pitch=vt_pitch)
+
+    def attention_core(self, name, qkv, out: Act, **kw):
+        """softmax(q k^T / sqrt(D)) v over the attention_operands `qkv` -> out ([B, S, heads * D] rows)."""
+        self._emit(ops.attention_op(name, self.lib_or_dry(), out=out.buf, batch=out.n, seq_q=qkv["q_rows"],
+                                    seq_kv=qkv["k_rows"], dt=self.dt, dry=self.dry, **qkv, **kw))
+
+    def conv_in(self, prefix, x, dst: Act):
+        """3x3 conv of the NCHW model input x (few channels, sfb_conv_in) -> NHWC dst."""
+        B, cin, H, W = x.shape
+        w = self.w.conv_in_weight(prefix + ".weight")
+        self._emit(Op(prefix, self.lib_or_dry().sfb_conv_in,
+                      (_ptr(x), _ptr(w), _ptr(self.w.f32(prefix + ".bias")), dst.ptr, B, H, W, cin, dst.c, dst.ld,
+                       ops.dtype_code(self.dt)), (x, w, dst.buf), 2 * B * H * W * dst.c * 9 * cin))
+
+    def conv_out(self, name, y: Act, w, bias, out, flops=None):
+        """3x3 conv of NHWC y to the few-channel NCHW model output `out` (sfb_conv_out); `w` packed like
+        PackedWeights.conv3x3_plain."""
+        cout = out.shape[1]
+        self._emit(Op(name, self.lib_or_dry().sfb_conv_out,
+                      (y.ptr, _ptr(w), _ptr(bias), _ptr(out), y.n, y.h, y.w, y.c, cout, y.ld, ops.dtype_code(self.dt)),
+                      (y.buf, w, bias, out), flops or 2 * y.rows * y.c * 9 * cout))
+
+    # ------------------------------------------------------------------ execution
+    def run(self, stream=None):
+        """Launch one step on torch's current stream (plus the forked side stream)."""
+        main = torch.cuda.current_stream()
+        mptr = main.cuda_stream
+        if self.side_ops:
+            if self._side_stream is None:
+                self._side_stream = torch.cuda.Stream()
+                self._temb_event = torch.cuda.Event()
+            side = self._side_stream
+            side.wait_stream(main)  # inputs were copied on the main stream
+            sptr = side.cuda_stream
+            for op in self.side_ops:
+                op.launch(sptr)
+                if op is self._temb_last:
+                    self._temb_event.record(side)
+        for op in self.ops:
+            if isinstance(op, _JoinOp):
+                if op.kind == "temb":
+                    main.wait_event(self._temb_event)
+                elif op.kind == "all":
+                    main.wait_stream(self._side_stream)
+                else:  # join of one forked branch
+                    main.wait_event(op.kind.ev_done)
+            elif isinstance(op, _ForkOp):
+                if op.ev_fork is None:
+                    op.ev_fork, op.ev_done = torch.cuda.Event(), torch.cuda.Event()
+                op.ev_fork.record(main)
+                side.wait_event(op.ev_fork)
+                for o in op.branch:
+                    o.launch(sptr)
+                op.ev_done.record(side)
+            else:
+                op.launch(mptr)
+
+    def all_ops(self):
+        """Every kernel-launching op of one step (markers removed, forked branches expanded)."""
+        out = list(self.side_ops)
+        for op in self.ops:
+            if isinstance(op, _ForkOp):
+                out.extend(op.branch)
+            elif not isinstance(op, _JoinOp):
+                out.append(op)
+        return out
+
+    def flops(self):
+        return sum(op.flops for op in self.all_ops())
+
+
+class UNetPlan(Plan):
+    """One static launch schedule of the UNet for a fixed (batch, height, width)."""
+
+    def __init__(self, weights: PackedWeights, batch, height, width, ctx_len=77, controlnet=False):
+        spec = weights.spec
+        div = 1 << (len(spec.block_out_channels) - 1)
+        if height % div or width % div:
+            # diffusers switches to explicit upsample sizes there (forward_upsample_size); not built
+            raise NotImplementedError(
+                f"sfast (H100 build): latent size {height}x{width} must be a multiple of {div}")
+        n_gn = sum(2 for _ in spec.all_resnets()) + 1 + sum(
+            1 for blk in spec.down + [spec.mid] + spec.up for t in blk.attentions if t is not None)
+        super().__init__(weights, batch, height, width, n_gn=n_gn,
+                         ln_floats=self._ln_arena_floats(spec, batch, height, width))
+        self.ctx_len = ctx_len
+        self.controlnet = controlnet
+        self.ctrl_in = []  # static NCHW inputs: 12 (SD-1.5) down-block residuals + the mid-block one
+        # ---- static inputs / output
+        self.sample_in = self._alloc((batch, spec.in_channels, height, width), self.dt)
+        self.t_in = self._alloc((batch,), torch.float32)
+        self.ehs_in = self._alloc((batch, ctx_len, spec.cross_attention_dim), self.dt)
+        self.out = self._alloc((batch, spec.out_channels, height, width), self.dt)
+        if spec.addition_embed_type == "text_time":
+            self.add_in = self._alloc((batch, spec.add_in_dim), self.dt)
+            self.time_ids_in = self._alloc((batch * 6,), torch.float32)
+        self._build()
+
+    @staticmethod
+    def _ln_arena_floats(spec, batch, height, width):
+        """3 * depth LayerNorms per transformer, each [B*h*w, slots(dim), 2] floats at its resolution."""
+        tot, h, w = 0, height, width
+
+        def need(blk):
+            return sum(3 * t.depth * batch * h * w * 2 * ops.rowstats_slots(t.dim)
+                       for t in blk.attentions if t is not None)
+        for blk in spec.down:
+            tot += need(blk)
+            if blk.sampler:
+                h, w = h // 2, w // 2
+        tot += need(spec.mid)
+        for blk in spec.up:
+            tot += need(blk)
+            if blk.sampler:
+                h, w = h * 2, w * 2
+        return tot
+
     # ------------------------------------------------------------------ sub-graphs
     def resnet(self, r, x: Act, dst: Act):
         p = r.prefix
@@ -513,22 +652,11 @@ class UNetPlan:
         projection (gamma-scaled weights + epilogue mean/rstd correction from `ln_stats`, the row
         sums the previous GEMM accumulated); `stats_next` receives the row sums of the new hs.
         Self-attention: fused QKV projection; cross: Q from the tokens, K/V from the text."""
-        B, S, C, H, D = hs.n, hs.h * hs.w, t.dim, t.heads, t.head_dim
-        dv = _round_up(D + 1, 16)  # + the all-ones row that yields the softmax denominator
-        q_pitch = _round_up(D, 64)
+        B, S, C = hs.n, hs.h * hs.w, t.dim
         a = f"{blk}.attn2" if cross else f"{blk}.attn1"
-        skv = self.ctx_len if cross else S
-        vt_pitch = _round_up(skv, 64)
-        tag = f"{B}x{H}x{S}x{skv}x{D}"
-        q = self.buf("attn_q_" + tag, (B * H * S, q_pitch))
-        kv_tag = tag + ("@" + a if cross else "")  # hoisted cross K/V: one buffer pair per layer
-        k = self.buf("attn_k_" + kv_tag, (B * H * skv, q_pitch))
-        new_vt = ("attn_vt_" + kv_tag, (B * H * dv, vt_pitch), self.dt) not in self._bufs
-        vt = self.buf("attn_vt_" + kv_tag, (B * H * dv, vt_pitch))
-        if new_vt and not self.dry:
-            vt.view(B * H, dv, vt_pitch)[:, D, :] = 1.0
-        qkv = dict(q=q, k=k, vt=vt, heads=H, head_dim=D, q_pitch=q_pitch, q_rows=S, k_rows=skv,
-                   vt_rows=dv, vt_pitch=vt_pitch)
+        # hoisted cross K/V: one buffer pair per layer
+        qkv = self.attention_operands(B, t.heads, S, self.ctx_len if cross else S, t.head_dim,
+                                      kv_tag="@" + a if cross else "")
         names = [f"{a}.to_q.weight"] if cross else [f"{a}.to_q.weight", f"{a}.to_k.weight",
                                                     f"{a}.to_v.weight"]
         wm, bias, colsum = self.w.ln_matrix(names, ln_prefix)
@@ -548,41 +676,22 @@ class UNetPlan:
                 self._joined = True
                 self._emit(_JoinOp("all"))
         ao = self.act("attn_out", hs.n, hs.h, hs.w, C)
-        self._emit(ops.attention_op(a + ".core", self.lib_or_dry(), q=q, k=k, vt=vt, out=ao.buf,
-                                    batch=B, heads=H, head_dim=D, seq_q=S, seq_kv=skv, q_rows=S,
-                                    k_rows=skv, vt_rows=dv, q_pitch=q_pitch, vt_pitch=vt_pitch,
-                                    dt=self.dt, dry=self.dry))
+        self.attention_core(a + ".core", qkv, ao)
         self.linear(a + ".to_out", ao, self.w.matrix(f"{a}.to_out.0.weight"),
                     self.w.f32(f"{a}.to_out.0.bias"), hs, residual=hs, rowstats_out=stats_next)
-
-    def layer_norm(self, name, x: Act, prefix):
-        y = self.act("ln_out", x.n, x.h, x.w, x.c)
-        self._emit(ops.ln_op(name, self.lib_or_dry(), x=x.buf, y=y.buf, rows=x.rows, c=x.c,
-                             gamma=self.w.f32(prefix + ".weight"), beta=self.w.f32(prefix + ".bias"),
-                             eps=1e-5, dt=self.dt))
-        return y
-
-    def ln_slot(self, rows, dim):
-        """[rows, slots, 2] fp32 (sum, sum of squares) statistics of one folded LayerNorm over `dim`
-        columns: every producer writes its own slots, the consumer adds them in order."""
-        slots = ops.rowstats_slots(dim)
-        off = self._ln_used
-        self._ln_used += rows * slots * 2
-        self._ln_slots.append((off, rows))
-        return ("ln_slot", off, rows, slots)
 
     def transformer(self, t, x: Act, dst: Act):
         p = t.prefix
         a1 = self.group_norm(p + ".norm", x, p + ".norm", False, 1e-6)
         hs = self.act("tf_hidden", x.n, x.h, x.w, t.dim)
-        st = self._ln_view(self.ln_slot(hs.rows, t.dim))
+        st = self.ln_slot(hs.rows, t.dim)
         self.linear(p + ".proj_in", a1, self.w.matrix(p + ".proj_in.weight"),
                     self.w.f32(p + ".proj_in.bias"), hs, rowstats_out=st)
         for d in range(t.depth):
             b = f"{p}.transformer_blocks.{d}"
-            st2 = self._ln_view(self.ln_slot(hs.rows, t.dim))
+            st2 = self.ln_slot(hs.rows, t.dim)
             self.attention(b + ".attn1", hs, b + ".norm1", st, b, t, cross=False, stats_next=st2)
-            st3 = self._ln_view(self.ln_slot(hs.rows, t.dim))
+            st3 = self.ln_slot(hs.rows, t.dim)
             self.attention(b + ".attn2", hs, b + ".norm2", st2, b, t, cross=True, stats_next=st3)
             gm, bp, inner, colsum = self.w.ln_geglu(b + ".ff.net.0.proj", b + ".norm3")
             ff = self.act("ff_act", x.n, x.h, x.w, inner)
@@ -591,7 +700,7 @@ class UNetPlan:
                                   bias=bp, epi=EPI_GEGLU, geglu_n_out=inner,
                                   ln=dict(rowstats=st3, colsum=colsum, eps=1e-5, dim=t.dim),
                                   keep=(hs.buf, ff.buf, gm, colsum)))
-            st = self._ln_view(self.ln_slot(hs.rows, t.dim)) if d + 1 < t.depth else None
+            st = self.ln_slot(hs.rows, t.dim) if d + 1 < t.depth else None
             self.linear(b + ".ff.out", ff, self.w.matrix(b + ".ff.net.2.weight"),
                         self.w.f32(b + ".ff.net.2.bias"), hs, residual=hs, rowstats_out=st)
         self.linear(p + ".proj_out", hs, self.w.matrix(p + ".proj_out.weight"),
@@ -627,7 +736,6 @@ class UNetPlan:
                            int(spec.flip_sin_to_cos), float(spec.freq_shift),
                            _ptr(tid), ad, ops.dtype_code(self.dt)),
                           (self.time_ids_in, tid)))
-            self._add_concat = (n_text, tid)
             h2 = self.buf("add_h", (B, spec.temb_dim))
             self._emit(Op("add_embedding.concat", lib.sfb_copy2d,
                           (_ptr(tid), _ptr(self.add_in) + 2 * n_text, B, 6 * ad, 6 * ad, spec.add_in_dim),
@@ -657,12 +765,6 @@ class UNetPlan:
     # ------------------------------------------------------------------ whole UNet
     def _build(self):
         spec, B, H, W, lib = self.spec, self.B, self.H, self.W, self.lib_or_dry()
-        self._ws_token = _WsToken()
-        self._emit(Op("gn_sync.zero", lib.sfb_memset,
-                      (_ptr(self.gn_sync), 0,
-                       self.gn_sync.numel() * 4), (self.gn_sync,)))
-        self._emit(Op("ln_stats.zero", lib.sfb_memset,
-                      (_ptr(self.ln_arena), 0, self.ln_arena.numel() * 4), (self.ln_arena,)))
         # the time-embedding chain only depends on the timestep: forked stream, joined before the
         # first resnet (its conv1 epilogue adds the projected embedding)
         n_main = len(self.ops)
@@ -683,7 +785,6 @@ class UNetPlan:
         pending = list(range(len(skip_shapes)))
         skip_dst = {}
         up_in = {}
-        cprev = spec.block_out_channels[-1]
         for i, blk in enumerate(spec.up):
             for j, r in enumerate(blk.resnets):
                 idx = pending.pop()
@@ -707,11 +808,7 @@ class UNetPlan:
                         self.w.f32("conv_in.bias"), x)
             self.ops[-1].flops = 2 * B * H * W * c0 * 9 * spec.in_channels  # algorithmic, not padded
         else:
-            w_in = self.w.conv_in_weight("conv_in.weight")
-            self._emit(Op("conv_in", lib.sfb_conv_in,
-                          (_ptr(self.sample_in), _ptr(w_in), _ptr(self.w.f32("conv_in.bias")),
-                           x.ptr, B, H, W, spec.in_channels, c0, x.ld, ops.dtype_code(self.dt)),
-                          (self.sample_in, w_in, x.buf), 2 * B * H * W * c0 * 9 * spec.in_channels))
+            self.conv_in("conv_in", self.sample_in, x)
         self._emit(_JoinOp("temb"))
         # ---- down path
         k = 1
@@ -787,74 +884,12 @@ class UNetPlan:
                 self.conv3x3(blk.sampler, up, blk.sampler, up_in[(i + 1, 0)][1])
         # ---- head
         y = self.group_norm("conv_norm_out", x, "conv_norm_out", True, spec.eps)
-        w_out = self.w.conv3x3_plain("conv_out.weight")
-        self._emit(Op("conv_out", lib.sfb_conv_out,
-                      (y.ptr, _ptr(w_out),
-                       _ptr(self.w.f32("conv_out.bias")),
-                       _ptr(self.out), B, H, W, c0, spec.out_channels,
-                       y.ld, ops.dtype_code(self.dt)), (y.buf, w_out, self.out),
-                      2 * B * H * W * c0 * 9 * spec.out_channels))
-        assert self._gn_count == self.gn_stats.shape[0], (self._gn_count, self.gn_stats.shape)
-        if self._pending is not None:  # nothing consumed the last deferred reduction
-            self._pending["p"].defer_finish = 0
-            self._pending = None
-        # ---- split-K workspace: allocate once at the largest requirement and patch the ops
-        self._ws_token.finalize(self)
-
-    # ------------------------------------------------------------------ execution
-    def run(self, stream=None):
-        """Launch one UNet step on torch's current stream (plus the forked side stream)."""
-        main = torch.cuda.current_stream()
-        mptr = main.cuda_stream
-        if self.side_ops:
-            if self._side_stream is None:
-                self._side_stream = torch.cuda.Stream()
-                self._temb_event = torch.cuda.Event()
-            side = self._side_stream
-            side.wait_stream(main)  # inputs were copied on the main stream
-            sptr = side.cuda_stream
-            for op in self.side_ops:
-                op.launch(sptr)
-                if op is self._temb_last:
-                    self._temb_event.record(side)
-        for op in self.ops:
-            if isinstance(op, _JoinOp):
-                if op.kind == "temb":
-                    main.wait_event(self._temb_event)
-                elif op.kind == "all":
-                    main.wait_stream(self._side_stream)
-                else:  # join of one forked branch
-                    main.wait_event(op.kind.ev_done)
-            elif isinstance(op, _ForkOp):
-                if op.ev_fork is None:
-                    op.ev_fork, op.ev_done = torch.cuda.Event(), torch.cuda.Event()
-                op.ev_fork.record(main)
-                side.wait_event(op.ev_fork)
-                for o in op.branch:
-                    o.launch(sptr)
-                op.ev_done.record(side)
-            else:
-                op.launch(mptr)
-
-    def all_ops(self):
-        """Every kernel-launching op of one step (markers removed, forked branches expanded)."""
-        out = list(self.side_ops)
-        for op in self.ops:
-            if isinstance(op, _ForkOp):
-                out.extend(op.branch)
-            elif not isinstance(op, _JoinOp):
-                out.append(op)
-        return out
-
-    def flops(self):
-        return sum(op.flops for op in self.all_ops())
+        self.conv_out("conv_out", y, self.w.conv3x3_plain("conv_out.weight"), self.w.f32("conv_out.bias"), self.out)
+        self._finish()
 
 
 class _WsToken:
     """Deferred split-K workspace: ops are created before the shared buffer size is known."""
-
-    def __init__(self):
-        self.users = []
 
     def numel(self):
         return 1 << 62
@@ -891,6 +926,9 @@ class _JoinOp(Op):
         super().__init__("join(side stream)", None, (), ())
         self.kind = kind
 
+    def launch(self, stream):
+        raise RuntimeError("join marker is handled by Plan.run")
+
 
 class _ForkOp(Op):
     """`branch` runs on the side stream, ordered after everything already on the main stream."""
@@ -901,10 +939,7 @@ class _ForkOp(Op):
         self.ev_fork = self.ev_done = None
 
     def launch(self, stream):
-        raise RuntimeError("fork marker is handled by UNetPlan.run")
-
-    def launch(self, stream):
-        raise RuntimeError("join marker is handled by UNetPlan.run")
+        raise RuntimeError("fork marker is handled by Plan.run")
 
 
 class _DryFn:

@@ -77,50 +77,58 @@ class _GraphedPlan:
             self.plan.run()
 
 
-class CompiledUNet:
-    """Callable with the signature of diffusers ``UNet2DConditionModel.forward``."""
+class _CompiledModule:
+    """What every compiled module shares: one packed copy of the weights and a cache of plans + CUDA graphs,
+    used under one lock.
 
-    def __init__(self, config, state_dict_fn, enable_cuda_graph=True, preserve_parameters=True):
-        self._config = config
+    Reference contract (preserve_parameters=True): an in-place parameter update is seen by the next call.
+    The packed weights are copies, so the parameters' version counters are compared on every call and the
+    copies refreshed in place when they moved."""
+
+    _what = "module"  # for log messages
+
+    def __init__(self, spec, state_dict_fn, enable_cuda_graph=True, preserve_parameters=True):
+        self.spec = spec
         self._state_dict_fn = state_dict_fn
         self.enable_cuda_graph = enable_cuda_graph
-        # reference contract (preserve_parameters=True): an in-place parameter update is seen by
-        # the next call.  The packed weights are copies, so the parameters' version counters are
-        # compared on every call and the copies refreshed in place when they moved.
         self.preserve_parameters = preserve_parameters
         self._weights = None
         self._param_refs = None
         self._param_versions = None
         self._cached = {}
         self._lock = threading.Lock()
-        self.spec = spec_from_config(config)
-        self.first_call_s = None  # wall time of the first call (packing + plan + capture)
+        self._warned = set()
 
-    # -- weights -------------------------------------------------------------------------
-    def _versions(self):
-        return [p._version for p in self._param_refs]
+    def _warn_once(self, what, msg, *args):
+        if what not in self._warned:
+            logger.warning(msg, *args)
+            self._warned.add(what)
 
-    def _ensure_weights(self, dtype, device):
-        if self._weights is None or self._weights.dtype != dtype or self._weights.device != device:
-            logger.info("Packing UNet weights for the H100 path (%s, %s)", dtype, device)
+    def _track(self, sd):
+        self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
+        self._param_versions = [t._version for t in self._param_refs]
+
+    def _weights_for(self, dtype, device):
+        """The packed weights for (dtype, device): packed on first use and re-packed when either changes (the
+        plans of the old copy are dropped); refreshed in place when the parameters' version counters moved.
+        The caller holds the lock and `device` is current."""
+        w = self._weights
+        if w is None or w.dtype != dtype or w.device != device:
+            logger.info("Packing %s weights for the H100 path (%s, %s)", self._what, dtype, device)
             sd = self._state_dict_fn()
             self._weights = PackedWeights(self.spec, sd, dtype, device)
-            self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
-            self._param_versions = self._versions()
+            self._track(sd)
             self._cached.clear()
-        elif self.preserve_parameters:
-            now = self._versions()
-            if now != self._param_versions:
-                logger.info("UNet parameters changed in place: refreshing the packed weights")
-                self._refresh_locked()
+        elif self.preserve_parameters and [t._version for t in self._param_refs] != self._param_versions:
+            logger.info("%s parameters changed in place: refreshing the packed weights", self._what)
+            self._refresh_locked()
         return self._weights
 
     def _refresh_locked(self):
         sd = self._state_dict_fn()
         torch.cuda.current_stream().synchronize()  # no replay may be reading the old values
         self._weights.refresh(sd)
-        self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
-        self._param_versions = self._versions()
+        self._track(sd)
 
     def rebind(self):
         """Re-pack the weights now (same device storage: plans and CUDA graphs stay valid).
@@ -130,6 +138,34 @@ class CompiledUNet:
             if self._weights is not None:
                 with torch.cuda.device(self._weights.device):
                     self._refresh_locked()
+
+    def _graphed(self, key, make_plan):
+        """The plan + graph cached under `key`, built by make_plan() on first use (caller holds the lock)."""
+        gp = self._cached.get(key)
+        if gp is None:
+            logger.info("Building %s launch plan for %s", self._what, key)
+            gp = _GraphedPlan(make_plan(), self.enable_cuda_graph)
+            self._cached[key] = gp
+        return gp
+
+
+def _install(m, name, compiled, fn):
+    """Replace m.<name> by fn, which carries the compiled object and its plan cache."""
+    fn.__self__ = m
+    fn._cached = compiled._cached
+    fn._compiled = compiled
+    setattr(m, name, fn)
+    return m
+
+
+class CompiledUNet(_CompiledModule):
+    """Callable with the signature of diffusers ``UNet2DConditionModel.forward``."""
+
+    _what = "UNet"
+
+    def __init__(self, config, state_dict_fn, enable_cuda_graph=True, preserve_parameters=True):
+        super().__init__(spec_from_config(config), state_dict_fn, enable_cuda_graph, preserve_parameters)
+        self.first_call_s = None  # wall time of the first call (packing + plan + capture)
 
     # -- forward -------------------------------------------------------------------------
     def _call_svd(self, sample, timestep, encoder_hidden_states, added_time_ids, return_dict=True):
@@ -147,13 +183,8 @@ class CompiledUNet:
             raise NotImplementedError("sfast (H100 build): SVD path needs a single-token encoder_hidden_states")
         with self._lock, torch.cuda.device(sample.device):
             t_first = time.perf_counter() if self.first_call_s is None else None
-            weights = self._ensure_weights(dtype, sample.device)
-            key = ("svd", B, H, W, dtype, sample.device.index)
-            gp = self._cached.get(key)
-            if gp is None:
-                logger.info("Building SVD UNet launch plan for %s", key)
-                gp = _GraphedPlan(SVDPlan(weights, B, H, W), self.enable_cuda_graph)
-                self._cached[key] = gp
+            weights = self._weights_for(dtype, sample.device)
+            gp = self._graphed(("svd", B, H, W, dtype, sample.device.index), lambda: SVDPlan(weights, B, H, W))
             plan = gp.plan
             plan.sample_in.copy_(sample.reshape(B * F_, -1, H, W), non_blocking=True)
             plan.ehs_in.copy_(encoder_hidden_states.repeat_interleave(F_, dim=0), non_blocking=True)
@@ -206,14 +237,9 @@ class CompiledUNet:
         # everything below (allocation, TMA maps, launches, capture) targets sample's device
         with self._lock, torch.cuda.device(sample.device):
             t_first = time.perf_counter() if self.first_call_s is None else None
-            weights = self._ensure_weights(dtype, sample.device)
-            key = (B, H, W, dtype, ctx_len, sample.device.index, controlnet)
-            gp = self._cached.get(key)
-            if gp is None:
-                logger.info("Building UNet launch plan for %s", key)
-                plan = UNetPlan(weights, B, H, W, ctx_len, controlnet=controlnet)
-                gp = _GraphedPlan(plan, self.enable_cuda_graph)
-                self._cached[key] = gp
+            weights = self._weights_for(dtype, sample.device)
+            gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index, controlnet),
+                               lambda: UNetPlan(weights, B, H, W, ctx_len, controlnet=controlnet))
             plan = gp.plan
             plan.sample_in.copy_(sample, non_blocking=True)
             plan.ehs_in.copy_(encoder_hidden_states, non_blocking=True)
@@ -313,49 +339,30 @@ def temporal_decoder(state_dict):
     return "post_quant_conv.weight" not in state_dict
 
 
-class CompiledVAE:
+class CompiledVAE(_CompiledModule):
     """`AutoencoderKL.decode(z, return_dict=True, generator=None)` and `encode(x, return_dict=True)` on the
-    native path.  Both share one packed copy of the weights, refreshed in place when the parameters'
-    version counters move, and one cache of plans + CUDA graphs keyed by (kind, B, H, W, dtype, device)."""
+    native path.  Both share one packed copy of the weights and one cache of plans + CUDA graphs keyed by
+    (kind, B, H, W, dtype, device)."""
+
+    _what = "VAE"
 
     def __init__(self, module, eager_decode, eager_encode, enable_cuda_graph=True):
         from .vae_plan import vae_spec_from_config
+        super().__init__(vae_spec_from_config(module.config), module.state_dict, enable_cuda_graph)
         # eager_decode / eager_encode None: that entry is not compiled (it stays the module's own)
-        self.spec = vae_spec_from_config(module.config)
-        self._module, self._state_dict_fn = module, module.state_dict
+        self._module = module
         self._eager, self._eager_encode = eager_decode, eager_encode
-        self.enable_cuda_graph = enable_cuda_graph
-        self._weights, self._param_refs, self._param_versions = None, None, None
-        self._cached = {}
-        self._lock = threading.Lock()
-        self._warned = set()
 
-    def _warn_once(self, what, msg, *args):
-        if what not in self._warned:
-            logger.warning(msg, *args)
-            self._warned.add(what)
-
-    def _graphed(self, kind, plan_cls, x):
-        """Plan + graph of `kind` for x's shape (caller holds the lock and x's device is current)."""
-        if self._weights is None or self._weights.dtype != x.dtype or self._weights.device != x.device:
-            sd = self._state_dict_fn()
-            self._weights = PackedWeights(self.spec, sd, x.dtype, x.device)
-            self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
-            self._param_versions = [t._version for t in self._param_refs]
-            self._cached.clear()
-        elif [t._version for t in self._param_refs] != self._param_versions:
-            sd = self._state_dict_fn()
-            torch.cuda.current_stream().synchronize()
-            self._weights.refresh(sd)
-            self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
-            self._param_versions = [t._version for t in self._param_refs]
+    def _step(self, kind, plan_cls, input_name, x):
+        """Copy x into the static input `input_name` of the plan of `kind` for x's shape, run it, return a
+        copy of its output."""
         B, _, H, W = x.shape
-        key = (kind, B, H, W, x.dtype, x.device.index)
-        gp = self._cached.get(key)
-        if gp is None:
-            gp = _GraphedPlan(plan_cls(self._weights, B, H, W), self.enable_cuda_graph)
-            self._cached[key] = gp
-        return gp
+        with self._lock, torch.cuda.device(x.device):
+            weights = self._weights_for(x.dtype, x.device)
+            gp = self._graphed((kind, B, H, W, x.dtype, x.device.index), lambda: plan_cls(weights, B, H, W))
+            getattr(gp.plan, input_name).copy_(x, non_blocking=True)
+            gp.step()
+            return gp.plan.out.clone()
 
     def decode(self, z, return_dict=True, generator=None):
         from .vae_plan import VAEDecodePlan
@@ -365,11 +372,7 @@ class CompiledVAE:
                             "path (the native decoder computes in fp16 / bf16)", z.dtype)
             return self._eager(z, return_dict=return_dict, generator=generator)
         require_sm90(z.device)
-        with self._lock, torch.cuda.device(z.device):
-            gp = self._graphed("decode", VAEDecodePlan, z)
-            gp.plan.z_in.copy_(z, non_blocking=True)
-            gp.step()
-            out = gp.plan.out.clone()
+        out = self._step("decode", VAEDecodePlan, "z_in", z)
         if not return_dict:
             return (out,)
         try:
@@ -392,11 +395,7 @@ class CompiledVAE:
                             "than %s) is left on the module's eager path", tile)
             return self._eager_encode(x, return_dict=return_dict)
         require_sm90(x.device)
-        with self._lock, torch.cuda.device(x.device):
-            gp = self._graphed("encode", VAEEncodePlan, x)
-            gp.plan.x_in.copy_(x, non_blocking=True)
-            gp.step()
-            moments = gp.plan.out.clone()
+        moments = self._step("encode", VAEEncodePlan, "x_in", x)
         out_cls, dist_cls = _latent_dist_classes()
         dist = dist_cls(moments)
         if not return_dict:
@@ -428,46 +427,77 @@ def compile_vae_module(m, enable_cuda_graph=True):
     if eager_decode is not None:
         def decode(z, return_dict=True, generator=None):
             return compiled.decode(z, return_dict=return_dict, generator=generator)
-
-        decode.__self__ = m
-        decode._cached = compiled._cached
-        decode._compiled = compiled
-        m.decode = decode
+        _install(m, "decode", compiled, decode)
     if eager_encode is not None:
         def encode(x, return_dict=True):
             return compiled.encode(x, return_dict=return_dict)
-
-        encode.__self__ = m
-        encode._cached = compiled._cached
-        encode._compiled = compiled
-        m.encode = encode
+        _install(m, "encode", compiled, encode)
     return m
 
 
-class CompiledTextEncoder:
-    """transformers ``CLIPTextModel`` / ``CLIPTextModelWithProjection`` forward on the native path: the
-    text encoders the reference traces and graphs
-    (/root/reference/src/sfast/compilers/diffusion_pipeline_compiler.py:93-112).  One plan + CUDA graph
-    per (batch, sequence length); outputs are fresh tensors."""
+class _CompiledClip(_CompiledModule):
+    """A CLIP tower's forward on the native path: one plan + CUDA graph per input shape, outputs are fresh
+    tensors.  Subclasses name the tower's first weight (its dtype is the one computed in), its static input
+    and its projection output."""
 
-    def __init__(self, config, state_dict_fn, eager_forward, with_projection, enable_cuda_graph=True):
-        from .clip_plan import clip_text_spec_from_config
-        self.spec = clip_text_spec_from_config(config, with_projection)
-        self._state_dict_fn, self._eager = state_dict_fn, eager_forward
+    _weight0 = _input = _embeds = _proj_output = None
+
+    def __init__(self, spec, config, state_dict_fn, eager_forward, with_projection, enable_cuda_graph=True):
+        super().__init__(spec, state_dict_fn, enable_cuda_graph)
+        self._eager = eager_forward
         self.with_projection = with_projection
-        self.enable_cuda_graph = enable_cuda_graph
-        self._weights, self._param_refs, self._param_versions = None, None, None
-        self._cached = {}
-        self._lock = threading.Lock()
-        self._warned = False
         rd = cfg_get(config, "return_dict", None)
         self._return_dict_default = True if rd is None else bool(rd)
 
-    def _route_eager(self, why, args, kwargs):
-        if not self._warned:
-            logger.warning("sfast (H100 build): text encoder call left on the module's eager path (%s)", why)
-            self._warned = True
-        return self._eager(*args, **kwargs)
+    def _route_eager(self, why, call):
+        self._warn_once("eager", "sfast (H100 build): %s call left on the module's eager path (%s)", self._what, why)
+        return self._eager(**call)
+
+    def _run(self, x, key, make_plan, call, output_hidden_states, return_dict):
+        if self._weights is None:
+            dtype = self._state_dict_fn()[self._weight0].dtype
+            if dtype not in (torch.float16, torch.bfloat16):
+                return self._route_eager(f"{dtype} weights: the native encoder computes in fp16 / bf16", call)
+        else:
+            dtype = self._weights.dtype
+        require_sm90(x.device)
+        with self._lock, torch.cuda.device(x.device):
+            weights = self._weights_for(dtype, x.device)
+            gp = self._graphed(key, lambda: make_plan(weights))
+            plan = gp.plan
+            getattr(plan, self._input).copy_(x, non_blocking=True)
+            gp.step()
+            last = plan.last_hidden_state.clone()
+            pooled = plan.pooled.clone()
+            embeds = getattr(plan, self._embeds).clone() if self.with_projection else None
+            hidden = tuple(h.clone() for h in plan.hidden_states()) if output_hidden_states else None
+        if return_dict is None:
+            return_dict = self._return_dict_default
+        if self.with_projection:
+            if not return_dict:
+                return tuple(v for v in (embeds, last, hidden) if v is not None)
+            return _clip_output(self._proj_output, **{self._embeds: embeds}, last_hidden_state=last,
+                                hidden_states=hidden)
+        if not return_dict:
+            return tuple(v for v in (last, pooled, hidden) if v is not None)
+        return _clip_output("BaseModelOutputWithPooling", last_hidden_state=last, pooler_output=pooled,
+                            hidden_states=hidden)
+
+
+class CompiledTextEncoder(_CompiledClip):
+    """transformers ``CLIPTextModel`` / ``CLIPTextModelWithProjection`` forward on the native path: the
+    text encoders the reference traces and graphs
+    (/root/reference/src/sfast/compilers/diffusion_pipeline_compiler.py:93-112).  One plan + CUDA graph
+    per (batch, sequence length)."""
+
+    _what = "text encoder"
+    _weight0, _input = "text_model.embeddings.token_embedding.weight", "ids_in"
+    _embeds, _proj_output = "text_embeds", "CLIPTextModelOutput"
+
+    def __init__(self, config, state_dict_fn, eager_forward, with_projection, enable_cuda_graph=True):
+        from .clip_plan import clip_text_spec_from_config
+        super().__init__(clip_text_spec_from_config(config, with_projection), config, state_dict_fn, eager_forward,
+                         with_projection, enable_cuda_graph)
 
     def __call__(self, input_ids=None, attention_mask=None, position_ids=None, output_attentions=None,
                  output_hidden_states=None, return_dict=None, **kwargs):
@@ -479,75 +509,25 @@ class CompiledTextEncoder:
         if input_ids is None:
             raise ValueError("You have to specify input_ids")
         if attention_mask is not None or position_ids is not None or output_attentions or kwargs:
-            return self._route_eager("attention_mask / position_ids / output_attentions / extra kwargs", (), call)
-        sd = None
-        if self._weights is None:
-            sd = self._state_dict_fn()
-            wdt = sd["text_model.embeddings.token_embedding.weight"].dtype
-            if wdt not in (torch.float16, torch.bfloat16):
-                return self._route_eager(f"{wdt} weights: the native encoder computes in fp16 / bf16", (), call)
+            return self._route_eager("attention_mask / position_ids / output_attentions / extra kwargs", call)
         ids = input_ids.view(-1, input_ids.shape[-1])
-        require_sm90(ids.device)
         B, S = ids.shape
-        with self._lock, torch.cuda.device(ids.device):
-            if self._weights is None:
-                wdt = sd["text_model.embeddings.token_embedding.weight"].dtype
-                self._weights = PackedWeights(self.spec, sd, wdt, ids.device)
-                self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
-                self._param_versions = [t._version for t in self._param_refs]
-            elif [t._version for t in self._param_refs] != self._param_versions:
-                sd = self._state_dict_fn()
-                torch.cuda.current_stream().synchronize()
-                self._weights.refresh(sd)
-                self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
-                self._param_versions = [t._version for t in self._param_refs]
-            key = (B, S, ids.device.index)
-            gp = self._cached.get(key)
-            if gp is None:
-                gp = _GraphedPlan(ClipTextPlan(self._weights, B, S), self.enable_cuda_graph)
-                self._cached[key] = gp
-            plan = gp.plan
-            plan.ids_in.copy_(ids, non_blocking=True)
-            gp.step()
-            last = plan.last_hidden_state.clone()
-            pooled = plan.pooled.clone()
-            embeds = plan.text_embeds.clone() if self.with_projection else None
-            hidden = tuple(h.clone() for h in plan.hidden_states()) if output_hidden_states else None
-        if return_dict is None:
-            return_dict = self._return_dict_default
-        if self.with_projection:
-            if not return_dict:
-                return tuple(v for v in (embeds, last, hidden) if v is not None)
-            return _clip_output("CLIPTextModelOutput", text_embeds=embeds, last_hidden_state=last,
-                                hidden_states=hidden)
-        if not return_dict:
-            return tuple(v for v in (last, pooled, hidden) if v is not None)
-        return _clip_output("BaseModelOutputWithPooling", last_hidden_state=last, pooler_output=pooled,
-                            hidden_states=hidden)
+        return self._run(ids, (B, S, ids.device.index), lambda w: ClipTextPlan(w, B, S), call,
+                         output_hidden_states, return_dict)
 
 
-class CompiledVisionEncoder:
+class CompiledVisionEncoder(_CompiledClip):
     """transformers ``CLIPVisionModel`` / ``CLIPVisionModelWithProjection`` forward on the native path (the
     SVD pipeline's image_encoder, reference :100-103).  One plan + CUDA graph per batch size."""
 
+    _what = "image encoder"
+    _weight0, _input = "vision_model.embeddings.patch_embedding.weight", "pixels_in"
+    _embeds, _proj_output = "image_embeds", "CLIPVisionModelOutput"
+
     def __init__(self, config, state_dict_fn, eager_forward, with_projection, enable_cuda_graph=True):
         from .clip_plan import clip_vision_spec_from_config
-        self.spec = clip_vision_spec_from_config(config, with_projection)
-        self._state_dict_fn, self._eager = state_dict_fn, eager_forward
-        self.with_projection = with_projection
-        self.enable_cuda_graph = enable_cuda_graph
-        self._weights, self._param_refs, self._param_versions = None, None, None
-        self._cached = {}
-        self._lock = threading.Lock()
-        self._warned = False
-        rd = cfg_get(config, "return_dict", None)
-        self._return_dict_default = True if rd is None else bool(rd)
-
-    def _route_eager(self, why, call):
-        if not self._warned:
-            logger.warning("sfast (H100 build): image encoder call left on the module's eager path (%s)", why)
-            self._warned = True
-        return self._eager(**call)
+        super().__init__(clip_vision_spec_from_config(config, with_projection), config, state_dict_fn,
+                         eager_forward, with_projection, enable_cuda_graph)
 
     def __call__(self, pixel_values=None, interpolate_pos_encoding=False, output_attentions=None,
                  output_hidden_states=None, return_dict=None, **kwargs):
@@ -564,67 +544,22 @@ class CompiledVisionEncoder:
         if tuple(pixel_values.shape[1:]) != (spec.channels, spec.image_size, spec.image_size):
             raise ValueError(f"Input image size {tuple(pixel_values.shape[2:])} doesn't match model "
                              f"({spec.image_size}*{spec.image_size}).")
-        sd = None
-        if self._weights is None:
-            sd = self._state_dict_fn()
-            wdt = sd["vision_model.embeddings.patch_embedding.weight"].dtype
-            if wdt not in (torch.float16, torch.bfloat16):
-                return self._route_eager(f"{wdt} weights: the native encoder computes in fp16 / bf16", call)
-        require_sm90(pixel_values.device)
+        # (the copy into the static input casts to the module's dtype, as the module does)
         B = pixel_values.shape[0]
-        with self._lock, torch.cuda.device(pixel_values.device):
-            if self._weights is None:
-                wdt = sd["vision_model.embeddings.patch_embedding.weight"].dtype
-                self._weights = PackedWeights(self.spec, sd, wdt, pixel_values.device)
-                self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
-                self._param_versions = [t._version for t in self._param_refs]
-            elif [t._version for t in self._param_refs] != self._param_versions:
-                sd = self._state_dict_fn()
-                torch.cuda.current_stream().synchronize()
-                self._weights.refresh(sd)
-                self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
-                self._param_versions = [t._version for t in self._param_refs]
-            key = (B, pixel_values.device.index)
-            gp = self._cached.get(key)
-            if gp is None:
-                gp = _GraphedPlan(ClipVisionPlan(self._weights, B), self.enable_cuda_graph)
-                self._cached[key] = gp
-            plan = gp.plan
-            plan.pixels_in.copy_(pixel_values, non_blocking=True)   # (casts to the module's dtype, as the module does)
-            gp.step()
-            last = plan.last_hidden_state.clone()
-            pooled = plan.pooled.clone()
-            embeds = plan.image_embeds.clone() if self.with_projection else None
-            hidden = tuple(h.clone() for h in plan.hidden_states()) if output_hidden_states else None
-        if return_dict is None:
-            return_dict = self._return_dict_default
-        if self.with_projection:
-            if not return_dict:
-                return tuple(v for v in (embeds, last, hidden) if v is not None)
-            return _clip_output("CLIPVisionModelOutput", image_embeds=embeds, last_hidden_state=last,
-                                hidden_states=hidden)
-        if not return_dict:
-            return tuple(v for v in (last, pooled, hidden) if v is not None)
-        return _clip_output("BaseModelOutputWithPooling", last_hidden_state=last, pooler_output=pooled,
-                            hidden_states=hidden)
+        return self._run(pixel_values, (B, pixel_values.device.index), lambda w: ClipVisionPlan(w, B), call,
+                         output_hidden_states, return_dict)
 
 
 def compile_image_encoder_module(m, enable_cuda_graph=True):
     """Replace ``m.forward`` of a CLIPVisionModel / CLIPVisionModelWithProjection (same module object)."""
-    with_projection = hasattr(m, "visual_projection")
-    eager = m.forward
-    compiled = CompiledVisionEncoder(m.config, m.state_dict, eager, with_projection, enable_cuda_graph)
+    compiled = CompiledVisionEncoder(m.config, m.state_dict, m.forward, hasattr(m, "visual_projection"),
+                                     enable_cuda_graph)
 
     def forward(*args, **kwargs):
         if args:
             kwargs = dict(zip(("pixel_values",), args), **kwargs)
         return compiled(**kwargs)
-
-    forward.__self__ = m
-    forward._cached = compiled._cached
-    forward._compiled = compiled
-    m.forward = forward
-    return m
+    return _install(m, "forward", compiled, forward)
 
 
 class _PlainOutput(dict):
@@ -654,20 +589,14 @@ def _clip_output(kind, **fields):
 
 def compile_text_encoder_module(m, enable_cuda_graph=True):
     """Replace ``m.forward`` of a CLIPTextModel / CLIPTextModelWithProjection (same module object)."""
-    with_projection = hasattr(m, "text_projection")
-    eager = m.forward
-    compiled = CompiledTextEncoder(m.config, m.state_dict, eager, with_projection, enable_cuda_graph)
+    compiled = CompiledTextEncoder(m.config, m.state_dict, m.forward, hasattr(m, "text_projection"),
+                                   enable_cuda_graph)
 
     def forward(*args, **kwargs):
         if args:
             kwargs = dict(zip(("input_ids", "attention_mask", "position_ids"), args), **kwargs)
         return compiled(**kwargs)
-
-    forward.__self__ = m
-    forward._cached = compiled._cached
-    forward._compiled = compiled
-    m.forward = forward
-    return m
+    return _install(m, "forward", compiled, forward)
 
 
 def compile_unet_module(m, enable_cuda_graph=True, preserve_parameters=True):
@@ -677,9 +606,4 @@ def compile_unet_module(m, enable_cuda_graph=True, preserve_parameters=True):
 
     def forward(*args, **kwargs):
         return compiled(*args, **kwargs)
-
-    forward.__self__ = m
-    forward._cached = compiled._cached
-    forward._compiled = compiled
-    m.forward = forward
-    return m
+    return _install(m, "forward", compiled, forward)

@@ -37,8 +37,10 @@ class SVDPlan(UNetPlan):
         super().__init__(weights, videos * self.F, height, width, ctx_len=1)
 
     # --------------------------------------------------------------------------- bookkeeping
-    def _ln_arena_floats(self):
-        return 2 * super()._ln_arena_floats()  # spatial + temporal blocks: <= 6 row-statistic slots per depth
+    @staticmethod
+    def _ln_arena_floats(spec, batch, height, width):
+        # spatial + temporal blocks: <= 6 row-statistic slots per depth
+        return 2 * UNetPlan._ln_arena_floats(spec, batch, height, width)
 
     def _alloc_extra_inputs(self):
         spec = self.spec
@@ -215,7 +217,7 @@ class SVDPlan(UNetPlan):
         a1 = self.group_norm(p + ".norm", x, p + ".norm", False, 1e-6)
         hs = self.act("tf_hidden", x.n, x.h, x.w, dim)
         hm = self.act("tf_mix", x.n, x.h, x.w, dim)
-        st = self._ln_view(self.ln_slot(hs.rows, dim))
+        st = self.ln_slot(hs.rows, dim)
         self.linear(p + ".proj_in", a1, self.w.matrix(p + ".proj_in.weight"), self.w.f32(p + ".proj_in.bias"),
                     hs, rowstats_out=st)
         pos = self.frame_pos_embedding(t)
@@ -226,15 +228,15 @@ class SVDPlan(UNetPlan):
             # ---- spatial block: self-attention per frame; cross-attention over one token = add
             self.attention(b + ".attn1", hs, b + ".norm1", st, b, t, cross=False, stats_next=None)
             self._join_side()
-            st3 = self._ln_view(self.ln_slot(hs.rows, dim))
+            st3 = self.ln_slot(hs.rows, dim)
             self._emit(self._row_op(b + ".attn2(ctx add)", lib.sfb_row_broadcast_add, x=hs, y=hs, vec=vec_s,
                                     ldv=dim, stats=st3, mode=_lib.ROW_IDX_DIV_MOD, div=S, mod=self.B))
             self._ff(b, "ff", b + ".norm3", hs, st3, None, dim)
             # ---- temporal block on hm = hs + frame position embedding
-            st_in = self._ln_view(self.ln_slot(hs.rows, dim))
+            st_in = self.ln_slot(hs.rows, dim)
             self._emit(self._row_op(tb + ".pos add", lib.sfb_row_broadcast_add, x=hs, y=hm, vec=pos, ldv=dim,
                                     stats=st_in, mode=_lib.ROW_IDX_DIV_MOD, div=S, mod=self.F))
-            st1 = self._ln_view(self.ln_slot(hs.rows, dim))
+            st1 = self.ln_slot(hs.rows, dim)
             self._ff(tb, "ff_in", tb + ".norm_in", hm, st_in, st1, dim)
             # self-attention across frames
             wm, bias, colsum = self.w.ln_matrix([f"{tb}.attn1.to_q.weight", f"{tb}.attn1.to_k.weight",
@@ -254,12 +256,12 @@ class SVDPlan(UNetPlan):
                           4 * hm.rows * dim * 2))
             self.linear(tb + ".attn1.to_out", ao, self.w.matrix(f"{tb}.attn1.to_out.0.weight"),
                         self.w.f32(f"{tb}.attn1.to_out.0.bias"), hm, residual=hm)
-            st3t = self._ln_view(self.ln_slot(hs.rows, dim))
+            st3t = self.ln_slot(hs.rows, dim)
             self._emit(self._row_op(tb + ".attn2(ctx add)", lib.sfb_row_broadcast_add, x=hm, y=hm, vec=vec_t,
                                     ldv=dim, stats=st3t, mode=_lib.ROW_IDX_TEMPORAL_CTX))
             self._ff(tb, "ff", tb + ".norm3", hm, st3t, None, dim)
             # ---- AlphaBlender
-            st = self._ln_view(self.ln_slot(hs.rows, dim)) if d + 1 < t.depth else None
+            st = self.ln_slot(hs.rows, dim) if d + 1 < t.depth else None
             self._emit(self._row_op(p + ".time_mixer", lib.sfb_alpha_blend, x=hs, y=hs, x2=hm,
                                     mix=self.w.f32(p + ".time_mixer.mix_factor"), stats=st))
         self.linear(p + ".proj_out", hs, self.w.matrix(p + ".proj_out.weight"),

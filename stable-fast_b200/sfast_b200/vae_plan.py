@@ -20,7 +20,7 @@ import torch
 
 from . import _lib, ops
 from .ops import Act, Op, _ptr
-from .plan import UNetPlan, _WsToken
+from .plan import Plan
 from .unet_spec import cfg_get
 
 
@@ -164,23 +164,9 @@ def vae_encoder_param_shapes(spec: VAESpec):
     return out
 
 
-class _VAEPlan(UNetPlan):
-    """What the VAE's decoder and encoder schedules share: plan state without a time embedding or folded
-    LayerNorms, and the GroupNorm-folded resnet and single-head attention sub-graphs."""
-
-    def _init_vae(self, weights, batch, height, width, n_gn):  # noqa: UNetPlan.__init__ is UNet-specific
-        self.controlnet, self.ctrl_in = False, []
-        self.w, self.spec = weights, weights.spec
-        self.dt, self.dev, self.dry = weights.dtype, weights.device, weights.dry
-        self.lib = None if self.dry else _lib.lib()
-        self.B, self.H, self.W, self.ctx_len = batch, height, width, 0
-        self.ops, self.side_ops = [], []
-        self._side_stream, self._pending, self._gn_ws_patches, self._joined = None, None, [], True
-        self._bufs, self._gn_count = {}, 0
-        self._alloc_gn(n_gn, batch)
-        self.ln_arena = self._alloc((2,), torch.float32)
-        self._ln_used, self._ln_slots = 0, []
-        self.ws, self._ws_need = None, 0
+class _VAEPlan(Plan):
+    """What the VAE's decoder and encoder schedules share: the GroupNorm-folded resnet and single-head
+    attention sub-graphs (no time embedding, no folded LayerNorms)."""
 
     def vae_resnet(self, p, x: Act, dst: Act, cin, cout):
         eps = self.spec.eps
@@ -238,8 +224,8 @@ class VAEDecodePlan(_VAEPlan):
 
     def __init__(self, weights, batch, height, width):
         spec = weights.spec
-        n_gn = 2 * (2 + len(spec.block_out_channels) * (spec.layers_per_block + 1)) + 2
-        self._init_vae(weights, batch, height, width, n_gn)
+        super().__init__(weights, batch, height, width,
+                         n_gn=2 * (2 + len(spec.block_out_channels) * (spec.layers_per_block + 1)) + 2)
         self.z_in = self._alloc((batch, spec.latent_channels, height, width), self.dt)
         up = 1 << (len(spec.block_out_channels) - 1)
         self.out = self._alloc((batch, spec.out_channels, height * up, width * up), self.dt)
@@ -247,9 +233,6 @@ class VAEDecodePlan(_VAEPlan):
 
     def _build(self):
         spec, B, H, W, lib = self.spec, self.B, self.H, self.W, self.lib_or_dry()
-        self._ws_token = _WsToken()
-        self._emit(Op("gn_sync.zero", lib.sfb_memset, (_ptr(self.gn_sync), 0, self.gn_sync.numel() * 4),
-                      (self.gn_sync,)))
         lc, boc = spec.latent_channels, spec.block_out_channels
         c = boc[-1]
         # post_quant_conv (1x1, NCHW -> NCHW) then conv_in (NCHW -> NHWC)
@@ -259,10 +242,7 @@ class VAEDecodePlan(_VAEPlan):
                       (_ptr(self.z_in), _ptr(wpq), _ptr(self.w.f32("post_quant_conv.bias")), _ptr(zq), B, H * W,
                        lc, lc, ops.dtype_code(self.dt)), (self.z_in, wpq, zq)))
         x = self.act("vae_x0", B, H, W, c)
-        w_in = self.w.conv_in_weight("decoder.conv_in.weight")
-        self._emit(Op("decoder.conv_in", lib.sfb_conv_in,
-                      (_ptr(zq), _ptr(w_in), _ptr(self.w.f32("decoder.conv_in.bias")), x.ptr, B, H, W, lc, c,
-                       x.ld, ops.dtype_code(self.dt)), (zq, w_in, x.buf), 2 * B * H * W * c * 9 * lc))
+        self.conv_in("decoder.conv_in", zq, x)
         m = "decoder.mid_block"
         a = self.act("vae_x1", B, H, W, c)
         self.vae_resnet(m + ".resnets.0", x, a, c, c)
@@ -281,16 +261,9 @@ class VAEDecodePlan(_VAEPlan):
                                f"decoder.up_blocks.{i}.upsamplers.0.conv", dst)
                 x, h, w = dst, 2 * h, 2 * w
         y = self.group_norm("decoder.conv_norm_out", x, "decoder.conv_norm_out", True, spec.eps)
-        w_out = self.w.conv3x3_plain("decoder.conv_out.weight")
-        self._emit(Op("decoder.conv_out", lib.sfb_conv_out,
-                      (y.ptr, _ptr(w_out), _ptr(self.w.f32("decoder.conv_out.bias")), _ptr(self.out), B, h, w,
-                       boc[0], spec.out_channels, y.ld, ops.dtype_code(self.dt)), (y.buf, w_out, self.out),
-                      2 * B * h * w * boc[0] * 9 * spec.out_channels))
-        assert self._gn_count <= self.gn_stats.shape[0], (self._gn_count, self.gn_stats.shape)
-        if self._pending is not None:
-            self._pending["p"].defer_finish = 0
-            self._pending = None
-        self._ws_token.finalize(self)
+        self.conv_out("decoder.conv_out", y, self.w.conv3x3_plain("decoder.conv_out.weight"),
+                      self.w.f32("decoder.conv_out.bias"), self.out)
+        self._finish()
 
 
 class VAEEncodePlan(_VAEPlan):
@@ -306,23 +279,17 @@ class VAEEncodePlan(_VAEPlan):
             raise NotImplementedError(
                 f"sfast (H100 build): VAE encode of a {height}x{width} image: the size must be a multiple of "
                 f"{div} with a latent of a multiple of 64 pixels")
-        self._init_vae(weights, batch, height, width, 2 * (2 + len(spec.block_out_channels) * spec.layers_per_block) + 2)
+        super().__init__(weights, batch, height, width,
+                         n_gn=2 * (2 + len(spec.block_out_channels) * spec.layers_per_block) + 2)
         self.x_in = self._alloc((batch, spec.in_channels, height, width), self.dt)
         self.out = self._alloc((batch, 2 * spec.latent_channels, height // div, width // div), self.dt)
         self._build()
 
     def _build(self):
-        spec, B, H, W, lib = self.spec, self.B, self.H, self.W, self.lib_or_dry()
-        self._ws_token = _WsToken()
-        self._emit(Op("gn_sync.zero", lib.sfb_memset, (_ptr(self.gn_sync), 0, self.gn_sync.numel() * 4),
-                      (self.gn_sync,)))
-        boc, cin_img, m = spec.block_out_channels, spec.in_channels, 2 * spec.latent_channels
-        # conv_in (NCHW -> NHWC)
+        spec, B, H, W = self.spec, self.B, self.H, self.W
+        boc, m = spec.block_out_channels, 2 * spec.latent_channels
         x = self.act("enc_x0", B, H, W, boc[0])
-        w_in = self.w.conv_in_weight("encoder.conv_in.weight")
-        self._emit(Op("encoder.conv_in", lib.sfb_conv_in,
-                      (_ptr(self.x_in), _ptr(w_in), _ptr(self.w.f32("encoder.conv_in.bias")), x.ptr, B, H, W, cin_img,
-                       boc[0], x.ld, ops.dtype_code(self.dt)), (self.x_in, w_in, x.buf), 2 * B * H * W * boc[0] * 9 * cin_img))
+        self.conv_in("encoder.conv_in", self.x_in, x)
         cout, h, w = boc[0], H, W
         for i, ch in enumerate(boc):
             cin, cout = cout, ch
@@ -344,11 +311,5 @@ class VAEEncodePlan(_VAEPlan):
         y = self.group_norm("encoder.conv_norm_out", a, "encoder.conv_norm_out", True, spec.eps)
         # conv_out then quant_conv (1x1) as ONE 3x3 conv with the folded weight (NHWC -> NCHW)
         w_out, b_out = self.w.conv3x3_pointwise("encoder.conv_out", "quant_conv")
-        self._emit(Op("encoder.conv_out+quant_conv", lib.sfb_conv_out,
-                      (y.ptr, _ptr(w_out), _ptr(b_out), _ptr(self.out), B, h, w, cout, m, y.ld, ops.dtype_code(self.dt)),
-                      (y.buf, w_out, b_out, self.out), 2 * B * h * w * m * (9 * cout + m)))
-        assert self._gn_count <= self.gn_stats.shape[0], (self._gn_count, self.gn_stats.shape)
-        if self._pending is not None:
-            self._pending["p"].defer_finish = 0
-            self._pending = None
-        self._ws_token.finalize(self)
+        self.conv_out("encoder.conv_out+quant_conv", y, w_out, b_out, self.out, flops=2 * B * h * w * m * (9 * cout + m))
+        self._finish()

@@ -24,6 +24,11 @@ sys.path.insert(0, _ROOT)  # oracle/ (the checker)
 from sfast_b200 import _lib, ops  # noqa: E402
 from sfast_b200.ops import Act  # noqa: E402
 
+# the fp32 F.conv2d / matmul references must not run in TF32 (cuDNN allows it by default): check_conv_gn's
+# normalised fp32 activations would be rounded to 10 mantissa bits inside the reference
+torch.backends.cudnn.allow_tf32 = False
+torch.backends.cuda.matmul.allow_tf32 = False
+
 DEV = "cuda"
 
 

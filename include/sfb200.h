@@ -127,7 +127,8 @@ enum sfb_epilogue {
     SFB_EPI_STORE_F32 = 3,
 };
 
-enum { SFB_ACT_NONE = 0, SFB_ACT_QUICK_GELU = 1 /* x * sigmoid(1.702 x) */, SFB_ACT_GELU = 2 /* erf form */ };
+enum { SFB_ACT_NONE = 0, SFB_ACT_QUICK_GELU = 1 /* x * sigmoid(1.702 x) */, SFB_ACT_GELU = 2 /* erf form */,
+       SFB_ACT_SILU = 3 /* x * sigmoid(x) */ };
 
 typedef struct sfb_gemm_params {
     const void* tmap_a; /* host pointer to a 128-byte tensor map */
@@ -409,6 +410,48 @@ typedef struct sfb_add_nchw_params {
 } sfb_add_nchw_params;
 
 int sfb_add_nchw_residuals(const sfb_add_nchw_params* p, sfb_stream_t stream);
+
+/* ---- ControlNet (diffusers ControlNetModel: a second UNet encoder plus the conditioning-image
+ * embedding; the reference leaves the module itself to eager PyTorch) ------------------------- */
+
+/* 3x3 convolution, zero padding 1 on every side, stride 1 or 2, for inputs with few channels (the
+ * conditioning embedding's layers at image resolution): y = act(conv(x) + bias), fp32 accumulation
+ * on mma.sync tensor cores, 16-bit storage.
+ *   x:      NCHW [n, cin, h, w] contiguous (x_nchw = 1, cin <= 8), or NHWC [n, h, w] with channel
+ *           pitch ldx (x_nchw = 0, cin < 64; cin and ldx multiples of 8);
+ *   weight: 16-bit [cout, 3, 3, cin16], cin16 = cin rounded up to 16, channels past cin zero;
+ *   bias:   fp32 [cout] or NULL;  silu: 1 applies SiLU after the bias;
+ *   y:      NHWC [n, ho, wo] with channel pitch ldy (ho = (h - 1) / stride + 1, likewise wo);
+ *           cout and ldy multiples of 8; only channels [0, cout) are written. */
+typedef struct sfb_conv_small_params {
+    const void* x;
+    const void* weight;
+    const float* bias;
+    void* y;
+    int32_t n, h, w, cin, cout, stride;
+    int32_t ldx, ldy;
+    int32_t x_nchw, silu, dtype;
+} sfb_conv_small_params;
+
+int sfb_conv3x3_small(const sfb_conv_small_params* p, sfb_stream_t stream);
+
+/* dst[n, c, hw] (NCHW contiguous) = scale[i] * src[n, hw, c] (NHWC, channel pitch ld_src) for item i,
+ * fp32 arithmetic, up to 16 tensors per launch (the ControlNet's down / mid residuals times
+ * conditioning_scale).  `scale` is a DEVICE fp32 array [count]: a captured graph serves every scale. */
+typedef struct sfb_nchw_scaled_item {
+    const void* src;
+    void* dst;
+    int32_t n, c, hw, ld_src;
+} sfb_nchw_scaled_item;
+
+typedef struct sfb_nhwc_to_nchw_params {
+    int32_t count;
+    int32_t dtype;
+    const float* scale;
+    sfb_nchw_scaled_item items[16];
+} sfb_nhwc_to_nchw_params;
+
+int sfb_nhwc_to_nchw_scaled(const sfb_nhwc_to_nchw_params* p, sfb_stream_t stream);
 
 /* dst[r, 0:cols] = src[r, 0:cols], 16-bit elements, row pitches in elements */
 int sfb_copy2d(const void* src, void* dst, int32_t rows, int32_t cols, int32_t ld_src,

@@ -49,11 +49,13 @@ class CompilationConfig:
 
 
 def compile(m, config):
-    """Compile a diffusers pipeline in place and return it (reference `compile`, :81-124)."""
+    """Compile a diffusers pipeline in place and return it (reference `compile`, :81-124): the UNet, the
+    ControlNet (``pipe.controlnet``: a ControlNetModel, or each net of a MultiControlNetModel), the VAE, the
+    text encoders and the image encoder run on the native path; a ControlNet class or config the native
+    path does not cover stays eager with a warning."""
     m.unet = compile_unet(m.unet, config)
     if getattr(m, 'controlnet', None) is not None:
-        logger.warning('sfast (H100 build): controlnet is left on its eager path '
-                       '(outside the UNet hot path, see DESIGN.md)')
+        m.controlnet = compile_controlnet(m.controlnet, config)
     if getattr(m, 'vae', None) is not None:
         m.vae = compile_vae(m.vae, config)
     # text encoders (reference :93-112: lazy trace + CUDA graph of text_encoder / text_encoder_2)
@@ -96,6 +98,37 @@ def compile_text_encoder(m, config):
         'cuda' if torch.cuda.is_available() else 'cpu')
     require_sm90(torch.device(device))
     return compile_text_encoder_module(m, enable_cuda_graph=bool(config.enable_cuda_graph))
+
+
+def compile_controlnet(m, config):
+    """Replace ``m.forward`` of a diffusers ControlNetModel with the H100-native ControlNet (the reference
+    compiles it like the UNet, :89-90).  A MultiControlNetModel (one with ``.nets``) gets each net's
+    forward replaced.  Any other class, or a config the native path does not cover, is left on its eager
+    path with a warning."""
+    nets = getattr(m, 'nets', None)
+    if nets is not None:
+        for net in nets:
+            _compile_controlnet_net(net, config)
+        return m
+    return _compile_controlnet_net(m, config)
+
+
+def _compile_controlnet_net(m, config):
+    from sfast_b200.runtime import compile_controlnet_module, require_sm90
+    from sfast_b200.unet_spec import controlnet_spec_from_config
+    if type(m).__name__ != 'ControlNetModel' or not hasattr(m, 'config'):
+        logger.warning('sfast (H100 build): %s is not a ControlNetModel; left on its eager path', type(m).__name__)
+        return m
+    try:
+        controlnet_spec_from_config(m.config)
+    except NotImplementedError as exc:
+        logger.warning('sfast (H100 build): ControlNet left on its eager path (%s)', exc)
+        return m
+    device = m.device if hasattr(m, 'device') else torch.device(
+        'cuda' if torch.cuda.is_available() else 'cpu')
+    require_sm90(torch.device(device))
+    return compile_controlnet_module(m, enable_cuda_graph=bool(config.enable_cuda_graph),
+                                     preserve_parameters=bool(getattr(config, 'preserve_parameters', True)))
 
 
 def compile_unet(m, config):

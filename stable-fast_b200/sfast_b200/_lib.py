@@ -15,7 +15,7 @@ SFB_F16, SFB_BF16 = 0, 1
 A_MATRIX, A_CONV3X3, A_UPCONV2X, A_CONV3X1, A_CONV3X3_GN, A_DOWNCONV3X3 = 0, 1, 2, 3, 4, 5
 ROW_IDX_DIV_MOD, ROW_IDX_TEMPORAL_CTX = 0, 1
 EPI_STORE, EPI_GEGLU, EPI_QKV, EPI_STORE_F32 = 0, 1, 2, 3
-ACT_NONE, ACT_QUICK_GELU, ACT_GELU = 0, 1, 2
+ACT_NONE, ACT_QUICK_GELU, ACT_GELU, ACT_SILU = 0, 1, 2, 3
 
 
 class GemmParams(C.Structure):
@@ -110,6 +110,22 @@ class AddNchwParams(C.Structure):
     _fields_ = [("count", C.c_int32), ("dtype", C.c_int32), ("items", AddNchwItem * 16)]
 
 
+class ConvSmallParams(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("weight", C.c_void_p), ("bias", C.c_void_p), ("y", C.c_void_p),
+                ("n", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("cin", C.c_int32), ("cout", C.c_int32),
+                ("stride", C.c_int32), ("ldx", C.c_int32), ("ldy", C.c_int32), ("x_nchw", C.c_int32),
+                ("silu", C.c_int32), ("dtype", C.c_int32)]
+
+
+class NchwScaledItem(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("n", C.c_int32), ("c", C.c_int32),
+                ("hw", C.c_int32), ("ld_src", C.c_int32)]
+
+
+class NhwcToNchwParams(C.Structure):
+    _fields_ = [("count", C.c_int32), ("dtype", C.c_int32), ("scale", C.c_void_p), ("items", NchwScaledItem * 16)]
+
+
 # every symbol include/sfb200.h declares: (name, restype, argtypes)
 _I32, _U32, _U64, _VP, _F = C.c_int32, C.c_uint32, C.c_uint64, C.c_void_p, C.c_float
 SYMBOLS = {
@@ -147,6 +163,8 @@ SYMBOLS = {
     "sfb_rowstats_slots": (C.c_int, [_I32]),
     "sfb_clip_pool": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _I32, _I32, _I32, _VP]),
     "sfb_patchify": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
+    "sfb_conv3x3_small": (C.c_int, [C.POINTER(ConvSmallParams), _VP]),
+    "sfb_nhwc_to_nchw_scaled": (C.c_int, [C.POINTER(NhwcToNchwParams), _VP]),
 }
 
 _lib = None

@@ -449,6 +449,33 @@ def small_linear_op(name, lib, *, x, w, bias, batch, n, k, dt, y16=None, y32=Non
               2 * batch * n * k, 2 * n * k)
 
 
+def conv_small_op(name, lib, *, x, weight, bias, y: Act, n, h, w, cin, cout, stride, dt, ldx=0, x_nchw=False,
+                  silu=False):
+    """sfb_conv3x3_small: 3x3 pad-1 conv of a few-channel input (NCHW tensor `x` when x_nchw, else an NHWC
+    buffer with channel pitch ldx) into the NHWC activation y; `weight` packed by
+    PackedWeights.conv3x3_small ([cout, 3, 3, cin16])."""
+    p = _lib.ConvSmallParams()
+    p.x, p.weight, p.bias, p.y = _ptr(x), _ptr(weight), _ptr(bias), y.ptr
+    p.n, p.h, p.w, p.cin, p.cout, p.stride = n, h, w, cin, cout, stride
+    p.ldx, p.ldy = ldx, y.ld
+    p.x_nchw, p.silu, p.dtype = int(bool(x_nchw)), int(bool(silu)), dtype_code(dt)
+    ho, wo = (h - 1) // stride + 1, (w - 1) // stride + 1
+    return Op(name, lib.sfb_conv3x3_small, (C.byref(p),), (p, x, weight, bias, y.buf),
+              2 * n * ho * wo * cout * 9 * cin, 2 * (n * h * w * cin + n * ho * wo * cout))
+
+
+def nhwc_to_nchw_scaled_op(name, lib, *, srcs, dsts, scale, dt):
+    """sfb_nhwc_to_nchw_scaled: dsts[i] (NCHW tensors) = scale[i] * srcs[i] (NHWC Acts), one launch."""
+    assert 0 < len(srcs) == len(dsts) <= 16
+    p = _lib.NhwcToNchwParams()
+    p.count, p.dtype, p.scale = len(srcs), dtype_code(dt), _ptr(scale)
+    for i, (s, d) in enumerate(zip(srcs, dsts)):
+        it = p.items[i]
+        it.src, it.dst, it.n, it.c, it.hw, it.ld_src = s.ptr, _ptr(d), s.n, s.c, s.h * s.w, s.ld
+    return Op(name, lib.sfb_nhwc_to_nchw_scaled, (C.byref(p),), (p, scale, [s.buf for s in srcs], list(dsts)),
+              0, sum(4 * d.numel() for d in dsts))
+
+
 # ---------------------------------------------------------------------------------------------
 # weight packing (done once at plan-build time)
 # ---------------------------------------------------------------------------------------------

@@ -241,6 +241,33 @@ class PackedWeights:
             return (self._mat(w), b)
         return self._get(("slin", prefix, scale), build)
 
+    def _padded_conv(self, name, cin_pad, cout_pad, flip_cin=False):
+        """[cout, cin, 3, 3] weight zero-padded to [cout_pad, cin_pad, 3, 3] (`flip_cin`: input channels in
+        reverse order -- a BGR conditioning image read as RGB)."""
+        w = self._raw(name).to(self.device)
+        if flip_cin:
+            w = w.flip(1)
+        return torch.nn.functional.pad(w, (0, 0, 0, 0, 0, cin_pad - w.shape[1], 0, cout_pad - w.shape[0]))
+
+    def conv3x3_small(self, name, cout_pad, flip_cin=False):
+        """3x3 conv weight for sfb_conv3x3_small: 16-bit [cout_pad, 3, 3, cin16], zero rows past cout and
+        zero input channels past cin."""
+        def build():
+            w = self._raw(name)
+            return ops.pack_conv3x3(self._padded_conv(name, _round_up(w.shape[1], 16), cout_pad, flip_cin),
+                                    self.dtype)
+        return self._get(("c3small", name, cout_pad, flip_cin), build)
+
+    def conv3x3_padded(self, name, cin_pad, cout_pad):
+        """3x3 conv weight zero-padded to cin_pad inputs and cout_pad outputs, as a GEMM operand."""
+        return self._get(("c3pad", name, cin_pad, cout_pad), lambda: self._mat(
+            ops.pack_conv3x3(self._padded_conv(name, cin_pad, cout_pad), self.dtype)))
+
+    def f32_padded(self, name, n):
+        """fp32 vector zero-padded to n entries."""
+        return self._get(("f32pad", name, n), lambda: torch.nn.functional.pad(
+            self._raw(name).to(device=self.device, dtype=torch.float32), (0, n - self._raw(name).shape[0])))
+
     def small(self, name):
         return self._get(("small", name), lambda: self._raw(name).to(
             device=self.device, dtype=self.dtype).contiguous())
@@ -405,12 +432,13 @@ class Plan:
         return x, dict(scale_shift=ab, silu=True)
 
     def conv3x3(self, name, x: Act, wname, dst: Act, stride=1, rowbias=None, residual: Act = None, gn=None,
-                down=False):
+                down=False, weights=None, act=0):
         """`down`: diffusers' Downsample2D with padding=0 (the VAE encoder's) -- stride 2, one zero row and
-        column AFTER the image, none before (SFB_A_DOWNCONV3X3)."""
+        column AFTER the image, none before (SFB_A_DOWNCONV3X3).  `weights`: a packed (Mat, fp32 bias) pair
+        used instead of the parameters `wname`; `act`: SFB_ACT_* of the epilogue (no split-K then)."""
         if down:
             stride = 2
-        wm = self.w.conv3x3(wname + ".weight")
+        wm = self.w.conv3x3(wname + ".weight") if weights is None else weights[0]
         cout = wm.n
         ho, wo = x.h // stride, x.w // stride
         if gn is not None:  # raw input, GroupNorm applied on the conv's operand path
@@ -422,10 +450,12 @@ class Plan:
             adesc = ops.a_conv(x.ptr, x.n, x.h, x.w, x.c, x.ld, box_n, box_h, box_w, stride)
         M = x.n * ho * wo
         kw = dict(a=adesc, b=wm, M=M, N=cout, K=9 * x.c, dt=self.dt,
-                  out=dst.ptr, ldo=dst.ld, bias=self.w.f32(wname + ".bias"),
+                  out=dst.ptr, ldo=dst.ld, bias=self.w.f32(wname + ".bias") if weights is None else weights[1],
                   conv=dict(n=x.n, h=ho, w=wo, cin=x.c, stride=stride, box_n=box_n, box_h=box_h,
                             box_w=box_w, down=down),
                   keep=(x.buf, dst.buf, wm))
+        if act:
+            kw.update(act=act, splits=1)
         if rowbias is not None:
             kw.update(rowbias=rowbias[0], rows_per_img=ho * wo, ld_rowbias=rowbias[1])
         if residual is not None:
@@ -577,7 +607,8 @@ class UNetPlan(Plan):
             # diffusers switches to explicit upsample sizes there (forward_upsample_size); not built
             raise NotImplementedError(
                 f"sfast (H100 build): latent size {height}x{width} must be a multiple of {div}")
-        n_gn = sum(2 for _ in spec.all_resnets()) + 1 + sum(
+        # (+1: conv_norm_out, the head of the up path; a ControlNet has none)
+        n_gn = sum(2 for _ in spec.all_resnets()) + (1 if spec.up else 0) + sum(
             1 for blk in spec.down + [spec.mid] + spec.up for t in blk.attentions if t is not None)
         super().__init__(weights, batch, height, width, n_gn=n_gn,
                          ln_floats=self._ln_arena_floats(spec, batch, height, width))
@@ -762,6 +793,21 @@ class UNetPlan(Plan):
                                        bias=self.w.tproj_b, batch=B, n=self.w.tproj_total,
                                        k=spec.temb_dim, dt=self.dt, y32=self.temb_proj))
 
+    def _sample_conv_in(self, x: Act):
+        """conv_in of the static NCHW input sample_in -> x (NHWC)."""
+        spec, B, H, W, lib = self.spec, self.B, self.H, self.W, self.lib_or_dry()
+        if spec.in_channels <= 7:
+            # im2col (K = 9*cin padded to one 64-wide K block) + the tcgen05 GEMM with fused bias
+            a_col = self.buf("conv_in_im2col", (B * H * W, 64))
+            self._emit(Op("conv_in.im2col", lib.sfb_im2col_in,
+                          (_ptr(self.sample_in), _ptr(a_col), B, H, W, spec.in_channels),
+                          (self.sample_in, a_col), 0, B * H * W * 128))
+            self.linear("conv_in", Act(a_col, B, H, W, 64), self.w.conv_in_matrix("conv_in.weight"),
+                        self.w.f32("conv_in.bias"), x)
+            self.ops[-1].flops = 2 * B * H * W * x.c * 9 * spec.in_channels  # algorithmic, not padded
+        else:
+            self.conv_in("conv_in", self.sample_in, x)
+
     # ------------------------------------------------------------------ whole UNet
     def _build(self):
         spec, B, H, W, lib = self.spec, self.B, self.H, self.W, self.lib_or_dry()
@@ -796,19 +842,8 @@ class UNetPlan(Plan):
         assert not pending
 
         # ---- conv_in
-        c0 = spec.block_out_channels[0]
         x = skip_dst[0]
-        if spec.in_channels <= 7:
-            # im2col (K = 9*cin padded to one 64-wide K block) + the tcgen05 GEMM with fused bias
-            a_col = self.buf("conv_in_im2col", (B * H * W, 64))
-            self._emit(Op("conv_in.im2col", lib.sfb_im2col_in,
-                          (_ptr(self.sample_in), _ptr(a_col), B, H, W, spec.in_channels),
-                          (self.sample_in, a_col), 0, B * H * W * 128))
-            self.linear("conv_in", Act(a_col, B, H, W, 64), self.w.conv_in_matrix("conv_in.weight"),
-                        self.w.f32("conv_in.bias"), x)
-            self.ops[-1].flops = 2 * B * H * W * c0 * 9 * spec.in_channels  # algorithmic, not padded
-        else:
-            self.conv_in("conv_in", self.sample_in, x)
+        self._sample_conv_in(x)
         self._emit(_JoinOp("temb"))
         # ---- down path
         k = 1

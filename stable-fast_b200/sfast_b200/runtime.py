@@ -599,6 +599,102 @@ def compile_text_encoder_module(m, enable_cuda_graph=True):
     return _install(m, "forward", compiled, forward)
 
 
+@functools.lru_cache(maxsize=None)
+def _controlnet_output_class():
+    """diffusers' ControlNetOutput where it imports, else a stand-in with attribute, key and index access."""
+    for mod in ("diffusers.models.controlnets.controlnet", "diffusers.models.controlnet"):
+        try:
+            return __import__(mod, fromlist=["ControlNetOutput"]).ControlNetOutput
+        except Exception:  # noqa: BLE001
+            pass
+    return ControlNetOutput
+
+
+class ControlNetOutput(dict):
+    """Stand-in for diffusers' ControlNetOutput (attribute, key and index access)."""
+
+    def __init__(self, down_block_res_samples, mid_block_res_sample):
+        super().__init__(down_block_res_samples=down_block_res_samples, mid_block_res_sample=mid_block_res_sample)
+        self.down_block_res_samples = down_block_res_samples
+        self.mid_block_res_sample = mid_block_res_sample
+
+    def __getitem__(self, k):
+        return tuple(self.values())[k] if isinstance(k, int) else super().__getitem__(k)
+
+    def to_tuple(self):
+        return tuple(self.values())
+
+
+class CompiledControlNet(_CompiledModule):
+    """Callable with the signature of diffusers ``ControlNetModel.forward``.  One plan + CUDA graph per
+    (batch, latent height, latent width, dtype, text length, device); conditioning_scale and guess mode are
+    inputs of the graph, not part of the key."""
+
+    _what = "ControlNet"
+
+    def __init__(self, config, state_dict_fn, enable_cuda_graph=True, preserve_parameters=True):
+        from .unet_spec import controlnet_spec_from_config
+        super().__init__(controlnet_spec_from_config(config), state_dict_fn, enable_cuda_graph, preserve_parameters)
+
+    def __call__(self, sample, timestep, encoder_hidden_states, controlnet_cond, conditioning_scale=1.0,
+                 class_labels=None, timestep_cond=None, attention_mask=None, added_cond_kwargs=None,
+                 cross_attention_kwargs=None, guess_mode=False, return_dict=True):
+        from .controlnet_plan import ControlNetPlan, residual_scales
+        given = dict(class_labels=class_labels, timestep_cond=timestep_cond, attention_mask=attention_mask)
+        for k, v in given.items():
+            if v is not None:
+                raise NotImplementedError(f"sfast (H100 build): ControlNet argument `{k}` is not supported")
+        if cross_attention_kwargs:
+            scale = cross_attention_kwargs.get("scale", 1.0)
+            if set(cross_attention_kwargs) - {"scale"} or scale != 1.0:
+                raise NotImplementedError("sfast (H100 build): cross_attention_kwargs (LoRA scale) "
+                                          "is not supported; fuse the LoRA weights into the parameters")
+        require_sm90(sample.device)
+        dtype = sample.dtype
+        if dtype not in (torch.float16, torch.bfloat16):
+            raise NotImplementedError(f"sfast (H100 build): ControlNet dtype {dtype}; use fp16 or bf16")
+        spec = self.spec
+        B, _, H, W = sample.shape
+        f = 1 << (len(spec.cond_embed_channels) - 1)
+        if tuple(controlnet_cond.shape) != (B, spec.cond_channels, f * H, f * W):
+            raise ValueError(f"controlnet_cond {tuple(controlnet_cond.shape)} must be {f}x the latent size: "
+                             f"expected {(B, spec.cond_channels, f * H, f * W)}")
+        ctx_len = encoder_hidden_states.shape[1]
+        with self._lock, torch.cuda.device(sample.device):
+            weights = self._weights_for(dtype, sample.device)
+            gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index),
+                               lambda: ControlNetPlan(weights, B, H, W, ctx_len))
+            plan = gp.plan
+            plan.sample_in.copy_(sample, non_blocking=True)
+            plan.ehs_in.copy_(encoder_hidden_states, non_blocking=True)
+            plan.cond_in.copy_(controlnet_cond, non_blocking=True)
+            plan.scale_in.copy_(residual_scales(len(plan.down_out), conditioning_scale, guess_mode))
+            t = timestep if torch.is_tensor(timestep) else torch.tensor(float(timestep))
+            t = t.reshape(-1).to(device=sample.device, dtype=torch.float32, non_blocking=True)
+            plan.t_in.copy_(t.expand(B) if t.numel() == 1 else t)
+            if spec.addition_embed_type == "text_time":
+                if not added_cond_kwargs or "text_embeds" not in added_cond_kwargs:
+                    raise ValueError("added_cond_kwargs with text_embeds / time_ids is required")
+                te = added_cond_kwargs["text_embeds"]
+                plan.add_in[:, :te.shape[1]].copy_(te)
+                plan.time_ids_in.copy_(added_cond_kwargs["time_ids"].reshape(-1).float())
+            gp.step()
+            down = tuple(o.clone() for o in plan.down_out)
+            mid = plan.mid_out.clone()
+        if not return_dict:
+            return down, mid
+        return _controlnet_output_class()(down_block_res_samples=down, mid_block_res_sample=mid)
+
+
+def compile_controlnet_module(m, enable_cuda_graph=True, preserve_parameters=True):
+    """Replace ``m.forward`` of a diffusers ControlNetModel (same module object)."""
+    compiled = CompiledControlNet(m.config, m.state_dict, enable_cuda_graph, preserve_parameters)
+
+    def forward(*args, **kwargs):
+        return compiled(*args, **kwargs)
+    return _install(m, "forward", compiled, forward)
+
+
 def compile_unet_module(m, enable_cuda_graph=True, preserve_parameters=True):
     """Replace ``m.forward`` (same module object, as the reference does at
     /root/reference/src/sfast/compilers/diffusion_pipeline_compiler.py:146-149)."""

@@ -84,6 +84,11 @@ class UNetSpec:
     mid: Optional[BlockSpec] = None
     up: List[BlockSpec] = field(default_factory=list)
     num_frames: int = 0     # > 0: UNetSpatioTemporalConditionModel (SVD)
+    # ControlNetModel (cond_channels > 0): conditioning image channels, the embedding's channel counts,
+    # and whether the image arrives in BGR order (controlnet_conditioning_channel_order)
+    cond_channels: int = 0
+    cond_embed_channels: tuple = ()
+    cond_bgr: bool = False
 
     @property
     def temporal(self):
@@ -99,6 +104,14 @@ class UNetSpec:
                     out.append(ResnetSpec(r.temporal_prefix, r.cout, r.cout, r.eps))
         return out
 
+    def residual_channels(self):
+        """Channels of the ControlNet's down-block residuals, in diffusers' order: conv_in's output, then
+        every resnet (+ transformer) output and every downsampler output of the down path."""
+        out = [self.block_out_channels[0]]
+        for b in self.down:
+            out += [b.cout] * len(b.resnets) + ([b.cout] if b.sampler else [])
+        return out
+
 
 _SUPPORTED_DOWN = ("CrossAttnDownBlock2D", "DownBlock2D")
 _SUPPORTED_UP = ("CrossAttnUpBlock2D", "UpBlock2D")
@@ -107,16 +120,41 @@ _SUPPORTED_UP = ("CrossAttnUpBlock2D", "UpBlock2D")
 def spec_from_config(cfg) -> UNetSpec:
     if is_svd_config(cfg):
         return svd_spec_from_config(cfg)
-    boc = tuple(cfg_get(cfg, "block_out_channels"))
-    nb = len(boc)
-    down_types = tuple(cfg_get(cfg, "down_block_types"))
+    spec, tf, layers = _encoder_spec(cfg, out_channels=cfg_get(cfg, "out_channels", 4))
     up_types = tuple(cfg_get(cfg, "up_block_types"))
-    for t in down_types:
-        if t not in _SUPPORTED_DOWN:
-            raise NotImplementedError(f"down block type {t} is not supported by the H100 path")
     for t in up_types:
         if t not in _SUPPORTED_UP:
             raise NotImplementedError(f"up block type {t} is not supported by the H100 path")
+    boc = spec.block_out_channels
+    nb = len(boc)
+    rboc = list(reversed(boc))
+    cout = rboc[0]
+    for i, t in enumerate(up_types):
+        cprev, cout = cout, rboc[i]
+        cin = rboc[min(i + 1, nb - 1)]
+        p = f"up_blocks.{i}"
+        res = []
+        for j in range(layers + 1):
+            skip = cin if j == layers else cout
+            rin = cprev if j == 0 else cout
+            res.append(ResnetSpec(f"{p}.resnets.{j}", rin + skip, cout))
+        att = [tf(f"{p}.attentions.{j}", cout, nb - 1 - i) if t.startswith("CrossAttn") else None
+               for j in range(layers + 1)]
+        spec.up.append(BlockSpec(p, res, att, f"{p}.upsamplers.0.conv" if i != nb - 1 else None,
+                                 cout))
+    return spec
+
+
+def _encoder_spec(cfg, out_channels):
+    """The part of the architecture a UNet and a ControlNet share (time embedding, conv_in, down blocks,
+    mid block), with every check of the config keys both carry.  Returns (spec without up blocks, the
+    transformer-spec factory, layers per block)."""
+    boc = tuple(cfg_get(cfg, "block_out_channels"))
+    nb = len(boc)
+    down_types = tuple(cfg_get(cfg, "down_block_types"))
+    for t in down_types:
+        if t not in _SUPPORTED_DOWN:
+            raise NotImplementedError(f"down block type {t} is not supported by the H100 path")
     for key in ("class_embed_type", "encoder_hid_dim_type", "time_cond_proj_dim",
                 "resnet_time_scale_shift", "dual_cross_attention", "only_cross_attention",
                 "upcast_attention", "time_embedding_act_fn", "attention_type"):
@@ -163,7 +201,7 @@ def spec_from_config(cfg) -> UNetSpec:
     if add_type not in (None, "text_time"):
         raise NotImplementedError(f"addition_embed_type={add_type}")
     spec = UNetSpec(
-        in_channels=cfg_get(cfg, "in_channels", 4), out_channels=cfg_get(cfg, "out_channels", 4),
+        in_channels=cfg_get(cfg, "in_channels", 4), out_channels=out_channels,
         block_out_channels=boc, temb_dim=boc[0] * 4, groups=cfg_get(cfg, "norm_num_groups", 32),
         eps=cfg_get(cfg, "norm_eps", 1e-5), flip_sin_to_cos=cfg_get(cfg, "flip_sin_to_cos", True),
         freq_shift=float(cfg_get(cfg, "freq_shift", 0)), cross_attention_dim=ctx,
@@ -188,21 +226,30 @@ def spec_from_config(cfg) -> UNetSpec:
                          [ResnetSpec("mid_block.resnets.0", c, c),
                           ResnetSpec("mid_block.resnets.1", c, c)],
                          [tf("mid_block.attentions.0", c, nb - 1)], None, c)
-    rboc = list(reversed(boc))
-    cout = rboc[0]
-    for i, t in enumerate(up_types):
-        cprev, cout = cout, rboc[i]
-        cin = rboc[min(i + 1, nb - 1)]
-        p = f"up_blocks.{i}"
-        res = []
-        for j in range(layers + 1):
-            skip = cin if j == layers else cout
-            rin = cprev if j == 0 else cout
-            res.append(ResnetSpec(f"{p}.resnets.{j}", rin + skip, cout))
-        att = [tf(f"{p}.attentions.{j}", cout, nb - 1 - i) if t.startswith("CrossAttn") else None
-               for j in range(layers + 1)]
-        spec.up.append(BlockSpec(p, res, att, f"{p}.upsamplers.0.conv" if i != nb - 1 else None,
-                                 cout))
+    return spec, tf, layers
+
+
+def controlnet_spec_from_config(cfg) -> UNetSpec:
+    """diffusers ``ControlNetModel``: the UNet's encoder half (``up = []``) plus the conditioning fields.
+    Every channel count of the conditioning embedding must be a multiple of 8 (the few-channel conv kernel
+    reads 8-channel vectors) and the conditioning image may have 1 to 8 channels."""
+    if cfg_get(cfg, "global_pool_conditions", False):
+        raise NotImplementedError("ControlNet config global_pool_conditions=True (shuffle models) is not "
+                                  "supported by the H100 path")
+    order = cfg_get(cfg, "controlnet_conditioning_channel_order", "rgb")
+    if order not in ("rgb", "bgr"):
+        raise NotImplementedError(f"ControlNet config controlnet_conditioning_channel_order={order!r} is not "
+                                  "supported by the H100 path (supported: 'rgb', 'bgr')")
+    cc = cfg_get(cfg, "conditioning_channels", 3)
+    if not 1 <= cc <= 8:
+        raise NotImplementedError(f"ControlNet config conditioning_channels={cc} is not supported by the H100 "
+                                  "path (supported: 1 to 8)")
+    emb = tuple(cfg_get(cfg, "conditioning_embedding_out_channels", (16, 32, 96, 256)))
+    if not emb or any(c <= 0 or c % 8 for c in emb) or emb[-1] < 64:
+        raise NotImplementedError(f"ControlNet config conditioning_embedding_out_channels={emb} is not supported "
+                                  "by the H100 path (every count a multiple of 8, the last one at least 64)")
+    spec, _, _ = _encoder_spec(cfg, out_channels=0)
+    spec.cond_channels, spec.cond_embed_channels, spec.cond_bgr = cc, emb, order == "bgr"
     return spec
 
 
@@ -392,6 +439,17 @@ def param_shapes(spec: UNetSpec):
                 transformer(t)
         if blk.sampler:
             conv(blk.sampler, blk.cout, blk.cout, 3)
+    if spec.cond_channels:
+        emb, e = spec.cond_embed_channels, "controlnet_cond_embedding"
+        conv(e + ".conv_in", emb[0], spec.cond_channels, 3)
+        for i in range(len(emb) - 1):
+            conv(f"{e}.blocks.{2 * i}", emb[i], emb[i], 3)
+            conv(f"{e}.blocks.{2 * i + 1}", emb[i + 1], emb[i], 3)
+        conv(e + ".conv_out", spec.block_out_channels[0], emb[-1], 3)
+        for i, c in enumerate(spec.residual_channels()):
+            conv(f"controlnet_down_blocks.{i}", c, c, 1)
+        conv("controlnet_mid_block", spec.mid.cout, spec.mid.cout, 1)
+        return out
     norm("conv_norm_out", spec.block_out_channels[0])
     conv("conv_out", spec.out_channels, spec.block_out_channels[0], 3)
     return out

@@ -20,6 +20,8 @@
  *                       csrc/operators/cutlass/cutlass_dual_linear_kernel.cu:442-539
  *                       (cutlass_linear_geglu_unified)
  *   sfb_attention       libs/xformers/xformers_attention.py:26-63 (memory_efficient_attention)
+ *   sfb_attention_ip    the same attention plus the IP-Adapter image-prompt term (the reference traces
+ *                       diffusers' IPAdapterAttnProcessor2_0 into two aten attention calls)
  *   sfb_group_norm_*    triton/ops/group_norm.py:126-165,272-320 (group_norm / group_norm_silu)
  *   sfb_layer_norm      triton/ops/layer_norm.py:51-133
  *   sfb_small_linear    csrc/operators/cublas/cublas_gemm.cpp:798-853 at M = batch rows
@@ -239,6 +241,26 @@ typedef struct sfb_attn_params {
 } sfb_attn_params;
 
 int sfb_attention(const sfb_attn_params* p, sfb_stream_t stream);
+
+/* Attention with an image prompt (diffusers' IPAdapterAttnProcessor2_0 of one IP-Adapter):
+ *   O = softmax(Q K^T * scale) V + s * softmax(Q K_ip^T * scale) V_ip,   s = *ip_scale
+ * `base` describes the text attention exactly as for sfb_attention.  K_ip / V_ip^T are laid out like K /
+ * V^T (the QKV-scatter epilogue writes them): K_ip [bh * k_ip_rows, q_pitch] through tmap_k_ip (box kv_tile
+ * rows), V_ip^T [bh * vt_rows, pitch >= kv_tile] through tmap_vt_ip (box vt_rows rows; the ones row of V^T
+ * is not needed).  Limits: 1 <= seq_ip <= kv_tile (the image tokens are one KV tile: n_img * 4 tokens up to
+ * 64 fit every head_dim), k_ip_rows >= seq_ip, no causal mask; every head_dim / kv_tile pair of
+ * sfb_attention, fp16 and bf16.  `ip_scale` is ONE fp32 value in DEVICE memory, so a captured graph serves
+ * every scale.  When it is 0 the image pass is skipped and the output is bit-identical to sfb_attention's
+ * on `base`. */
+typedef struct sfb_attn_ip_params {
+    sfb_attn_params base;
+    const void* tmap_k_ip;
+    const void* tmap_vt_ip;
+    int32_t seq_ip, k_ip_rows;
+    const float* ip_scale;
+} sfb_attn_ip_params;
+
+int sfb_attention_ip(const sfb_attn_ip_params* p, sfb_stream_t stream);
 
 /* ---- normalisation ----------------------------------------------------------------------- */
 

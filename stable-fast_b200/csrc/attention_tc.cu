@@ -16,6 +16,9 @@
 // [head_dim, seq] -- the QKV projection's epilogue (gemm_tc.cu, SFB_EPI_QKV) writes those
 // layouts directly, so no permute/copy kernels exist between projection and attention.
 //
+// attention_ip_kernel (sfb_attention_ip) is the same body with IP-Adapter's image-prompt term added after the
+// text tiles: O + s * softmax(Q K_ip^T * scale) V_ip, the image tokens being one more KV tile.
+//
 // Replaces xformers.ops.memory_efficient_attention as wrapped at
 // /root/reference/src/sfast/libs/xformers/xformers_attention.py:26-63.
 #include "common.cuh"
@@ -94,13 +97,19 @@ struct AttnSmem {
     static_assert(kTotal <= 227 * 1024, "shared memory per block");
 };
 
-// HD = head_dim (DK: HD rounded up to 16)
-template <int DC, int HD, int DK, int DV, int KV, int KVS, int BF16>
-// 9 warps: three share an SM sub-partition's 64 KB register file, hence at most 168 registers
-__global__ void __maxnreg__(168)  // kAttnThreads threads, one CTA per SM
-attention_tc_kernel(const __grid_constant__ CUtensorMap tma_q,
-                    const __grid_constant__ CUtensorMap tma_k,
-                    const __grid_constant__ CUtensorMap tma_vt, const AttnArgs a) {
+// Image-prompt (IP-Adapter) term of sfb_attention_ip: one more key / value set of at most one KV tile,
+// attended with its own softmax and added as `*scale` times its output.
+struct IpArgs {
+    int seq_ip, k_ip_rows;
+    const float* scale;  // device memory: a captured graph serves every scale
+};
+
+// HD = head_dim (DK: HD rounded up to 16).  IP: the image-prompt pass after the text tiles (below).
+template <int DC, int HD, int DK, int DV, int KV, int KVS, int BF16, bool IP>
+__device__ __forceinline__ void attention_body(const CUtensorMap* tma_q, const CUtensorMap* tma_k,
+                                               const CUtensorMap* tma_vt, const AttnArgs& a,
+                                               const CUtensorMap* tma_k_ip, const CUtensorMap* tma_vt_ip,
+                                               const IpArgs& ip) {
     using L = AttnSmem<DC, DV, KV, KVS>;
     constexpr unsigned kPolyMask = KV == 128 ? kPolyMaskV1 : kPolyMaskV2;
     extern __shared__ uint8_t smem_raw[];
@@ -122,9 +131,13 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tma_q,
     const int n_kv = (a.seq_kv + KV - 1) / KV;
 
     if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tma_q);
-        tma_prefetch_desc(&tma_k);
-        tma_prefetch_desc(&tma_vt);
+        tma_prefetch_desc(tma_q);
+        tma_prefetch_desc(tma_k);
+        tma_prefetch_desc(tma_vt);
+        if constexpr (IP) {
+            tma_prefetch_desc(tma_k_ip);
+            tma_prefetch_desc(tma_vt_ip);
+        }
         mbar_init(q_full, 1);
         for (int i = 0; i < KVS; ++i) {
             mbar_init(&k_full[i], 1);
@@ -145,7 +158,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tma_q,
             mbar_expect_tx(q_full, L::kQBytes);
 #pragma unroll
             for (int c = 0; c < DC; ++c)
-                tma_load_2d(sQ + c * (kTileQ * 128), &tma_q, q_full, c * 64, bh * a.q_rows + q_tile * kTileQ);
+                tma_load_2d(sQ + c * (kTileQ * 128), tma_q, q_full, c * 64, bh * a.q_rows + q_tile * kTileQ);
             for (int j = 0; j < n_kv; ++j) {
                 const int st = j % KVS;
                 const uint32_t ph = (j / KVS) & 1;
@@ -153,14 +166,34 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tma_q,
                 mbar_expect_tx(&k_full[st], L::kKStage);
 #pragma unroll
                 for (int c = 0; c < DC; ++c)
-                    tma_load_2d(sK + st * L::kKStage + c * (KV * 128), &tma_k, &k_full[st], c * 64,
+                    tma_load_2d(sK + st * L::kKStage + c * (KV * 128), tma_k, &k_full[st], c * 64,
                                 bh * a.k_rows + j * KV);
                 mbar_wait(&v_empty[st], ph ^ 1);
                 mbar_expect_tx(&v_full[st], L::kVStage);
 #pragma unroll
                 for (int c = 0; c < KV / 64; ++c)
-                    tma_load_2d(sV + st * L::kVStage + c * L::kVChunk, &tma_vt, &v_full[st], j * KV + c * 64,
+                    tma_load_2d(sV + st * L::kVStage + c * L::kVChunk, tma_vt, &v_full[st], j * KV + c * 64,
                                 bh * a.vt_rows);
+            }
+            // image-prompt keys / values: one more ring iteration (skipped, like the consumers' pass,
+            // when the scale is 0)
+            if constexpr (IP) {
+                if (*ip.scale != 0.f) {
+                    const int st = n_kv % KVS;
+                    const uint32_t ph = (n_kv / KVS) & 1;
+                    mbar_wait(&k_empty[st], ph ^ 1);
+                    mbar_expect_tx(&k_full[st], L::kKStage);
+#pragma unroll
+                    for (int c = 0; c < DC; ++c)
+                        tma_load_2d(sK + st * L::kKStage + c * (KV * 128), tma_k_ip, &k_full[st], c * 64,
+                                    bh * ip.k_ip_rows);
+                    mbar_wait(&v_empty[st], ph ^ 1);
+                    mbar_expect_tx(&v_full[st], L::kVStage);
+#pragma unroll
+                    for (int c = 0; c < KV / 64; ++c)
+                        tma_load_2d(sV + st * L::kVStage + c * L::kVChunk, tma_vt_ip, &v_full[st], c * 64,
+                                    bh * a.vt_rows);
+                }
             }
         }
     } else {
@@ -276,10 +309,86 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tma_q,
                 l[1] = (hd & 1) ? o[4 * jj + 3] : o[4 * jj + 2];
             }
         const int src = (lane & ~3) | ((hd & 7) >> 1);
+        float inv_l[2];
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh) inv_l[rh] = 1.0f / __shfl_sync(0xffffffffu, l[rh], src);
+        if constexpr (IP) {
+            // O = O_text / l + s * softmax(Q K_ip^T * scale) V_ip.  The text output is normalised in fp32
+            // first (the same product the plain store rounds), then the image term is added on the tensor
+            // core with its probabilities pre-multiplied by s / l_ip: no second accumulator.  s == 0 skips
+            // the pass, so the stored bits are exactly sfb_attention's.
+            const float s_ip = *ip.scale;
+            if (s_ip != 0.f) {
+                const int st = n_kv % KVS;
+                const uint32_t ph = (n_kv / KVS) & 1;
+                float s[KV / 2];
+#pragma unroll
+                for (int i = 0; i < KV / 2; ++i) s[i] = 0.f;
+                mbar_wait(&k_full[st], ph);
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < DK / 16; ++kk) {
+                    const int c = kk / 4, k4 = kk % 4;
+                    const uint64_t dq = wgmma_desc_k_sw128(smem_u32(sQ + c * (kTileQ * 128) + wg * 64 * 128));
+                    const uint64_t dk = wgmma_desc_k_sw128(smem_u32(sK + st * L::kKStage + c * (KV * 128)));
+                    wgmma_ss<BF16>(s, dq + (uint64_t)(k4 * 2), dk + (uint64_t)(k4 * 2));
+                }
+                wgmma_commit();
+                wgmma_wait<0>(s);
+                // columns >= seq_ip: the next (batch, head)'s rows or TMA zero fill
+                if (ip.seq_ip < KV) {
+#pragma unroll
+                    for (int i = 0; i < KV / 2; ++i)
+                        if ((i / 4) * 8 + qcol + (i & 1) >= ip.seq_ip) s[i] = -INFINITY;
+                }
+                float neg_m[2], l_ip[2] = {0.f, 0.f};
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float mx = -INFINITY;
+#pragma unroll
+                    for (int jj = 0; jj < KV / 8; ++jj) mx = fmax3(mx, s[4 * jj + 2 * h], s[4 * jj + 2 * h + 1]);
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                    neg_m[h] = -mx * sl2;  // column 0 is always valid: finite
+                }
+#pragma unroll
+                for (int i = 0; i < KV / 2; ++i) {
+                    s[i] = fast_exp2(fmaf(s[i], sl2, neg_m[(i >> 1) & 1]));
+                    l_ip[(i >> 1) & 1] += s[i];
+                }
+                float f[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    l_ip[h] += __shfl_xor_sync(0xffffffffu, l_ip[h], 1);
+                    l_ip[h] += __shfl_xor_sync(0xffffffffu, l_ip[h], 2);
+                    f[h] = s_ip / l_ip[h];
+                }
+                uint32_t pa[KV / 16][4];
+#pragma unroll
+                for (int kc = 0; kc < KV / 16; ++kc)
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) {
+                        const int i = 8 * kc + 2 * r;
+                        pa[kc][r] = pack2(s[i] * f[r & 1], s[i + 1] * f[r & 1], BF16);
+                    }
+#pragma unroll
+                for (int i = 0; i < DV / 2; ++i) o[i] *= inv_l[(i >> 1) & 1];
+                mbar_wait(&v_full[st], ph);
+                wgmma_fence();
+#pragma unroll
+                for (int kc = 0; kc < KV / 16; ++kc) {
+                    const int c = kc / 4, k4 = kc % 4;
+                    const uint64_t dv = wgmma_desc_k_sw128(smem_u32(sV + st * L::kVStage + c * L::kVChunk));
+                    wgmma_rs<BF16>(o, pa[kc], dv + (uint64_t)(k4 * 2));
+                }
+                wgmma_commit();
+                wgmma_wait<0>(o);
+                inv_l[0] = inv_l[1] = 1.f;
+            }
+        }
         const int b = bh / a.heads, h = bh % a.heads;
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh) {
-            const float inv_l = 1.0f / __shfl_sync(0xffffffffu, l[rh], src);
             const int srow = q_tile * kTileQ + row_g + 8 * rh;
             if (srow < a.seq_q) {
                 uint16_t* orow = reinterpret_cast<uint16_t*>(a.out) + ((size_t)b * a.seq_q + srow) * (a.heads * hd) +
@@ -288,22 +397,45 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tma_q,
                 for (int jj = 0; jj < DV / 8; ++jj)
                     if (jj * 8 < hd)
                         *reinterpret_cast<uint32_t*>(orow + jj * 8) =
-                            pack2(o[4 * jj + 2 * rh] * inv_l, o[4 * jj + 2 * rh + 1] * inv_l, BF16);
+                            pack2(o[4 * jj + 2 * rh] * inv_l[rh], o[4 * jj + 2 * rh + 1] * inv_l[rh], BF16);
             }
         }
     }
 }
 
+// 9 warps: three share an SM sub-partition's 64 KB register file, hence at most 168 registers
 template <int DC, int HD, int DK, int DV, int KV, int KVS, int BF16>
-static int launch_attention_t(const sfb_attn_params* p, const AttnArgs& a, cudaStream_t stream) {
+__global__ void __maxnreg__(168)  // kAttnThreads threads, one CTA per SM
+attention_tc_kernel(const __grid_constant__ CUtensorMap tma_q,
+                    const __grid_constant__ CUtensorMap tma_k,
+                    const __grid_constant__ CUtensorMap tma_vt, const AttnArgs a) {
+    attention_body<DC, HD, DK, DV, KV, KVS, BF16, false>(&tma_q, &tma_k, &tma_vt, a, nullptr, nullptr, IpArgs{});
+}
+
+template <int DC, int HD, int DK, int DV, int KV, int KVS, int BF16>
+__global__ void __maxnreg__(168)
+attention_ip_kernel(const __grid_constant__ CUtensorMap tma_q,
+                    const __grid_constant__ CUtensorMap tma_k,
+                    const __grid_constant__ CUtensorMap tma_vt, const AttnArgs a,
+                    const __grid_constant__ CUtensorMap tma_k_ip,
+                    const __grid_constant__ CUtensorMap tma_vt_ip, const IpArgs ip) {
+    attention_body<DC, HD, DK, DV, KV, KVS, BF16, true>(&tma_q, &tma_k, &tma_vt, a, &tma_k_ip, &tma_vt_ip, ip);
+}
+
+template <int DC, int HD, int DK, int DV, int KV, int KVS, int BF16, bool IP>
+static int launch_attention_t(const sfb_attn_params* p, const sfb_attn_ip_params* ipp, const AttnArgs& a,
+                              cudaStream_t stream) {
     using L = AttnSmem<DC, DV, KV, KVS>;
+    const char* what = IP ? "sfb_attention_ip" : "sfb_attention";
     static PerDeviceOnce attr_once;
     bool& attr_set = attr_once.flag();
     if (!attr_set) {
-        cudaError_t err = cudaFuncSetAttribute(attention_tc_kernel<DC, HD, DK, DV, KV, KVS, BF16>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal);
+        cudaError_t err = IP ? cudaFuncSetAttribute(attention_ip_kernel<DC, HD, DK, DV, KV, KVS, BF16>,
+                                                    cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal)
+                             : cudaFuncSetAttribute(attention_tc_kernel<DC, HD, DK, DV, KV, KVS, BF16>,
+                                                    cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal);
         if (err != cudaSuccess)
-            return fail(SFB_ERR_CUDA, "sfb_attention: smem attribute: %s", cudaGetErrorString(err));
+            return fail(SFB_ERR_CUDA, "%s: smem attribute: %s", what, cudaGetErrorString(err));
         attr_set = true;
     }
     CUtensorMap tq, tk, tv;
@@ -311,33 +443,43 @@ static int launch_attention_t(const sfb_attn_params* p, const AttnArgs& a, cudaS
     memcpy(&tk, p->tmap_k, sizeof(CUtensorMap));
     memcpy(&tv, p->tmap_vt, sizeof(CUtensorMap));
     dim3 grid((p->seq_q + kTileQ - 1) / kTileQ, p->batch * p->heads);
-    cudaError_t err = launch_pdl(attention_tc_kernel<DC, HD, DK, DV, KV, KVS, BF16>, grid, dim3(kAttnThreads),
-                                 L::kTotal, stream, tq, tk, tv, a);
-    if (err != cudaSuccess) return fail(SFB_ERR_CUDA, "sfb_attention: launch: %s", cudaGetErrorString(err));
-    return check_launch("sfb_attention");
+    cudaError_t err;
+    if constexpr (IP) {
+        CUtensorMap tk_ip, tv_ip;
+        memcpy(&tk_ip, ipp->tmap_k_ip, sizeof(CUtensorMap));
+        memcpy(&tv_ip, ipp->tmap_vt_ip, sizeof(CUtensorMap));
+        const IpArgs ip{ipp->seq_ip, ipp->k_ip_rows, ipp->ip_scale};
+        err = launch_pdl(attention_ip_kernel<DC, HD, DK, DV, KV, KVS, BF16>, grid, dim3(kAttnThreads), L::kTotal,
+                         stream, tq, tk, tv, a, tk_ip, tv_ip, ip);
+    } else {
+        err = launch_pdl(attention_tc_kernel<DC, HD, DK, DV, KV, KVS, BF16>, grid, dim3(kAttnThreads), L::kTotal,
+                         stream, tq, tk, tv, a);
+    }
+    if (err != cudaSuccess) return fail(SFB_ERR_CUDA, "%s: launch: %s", what, cudaGetErrorString(err));
+    return check_launch(what);
 }
 
-template <int DC, int HD, int DK, int DV, int KV, int KVS>
-static int launch_attention(const sfb_attn_params* p, const AttnArgs& a, cudaStream_t stream) {
-    return a.dtype == SFB_BF16 ? launch_attention_t<DC, HD, DK, DV, KV, KVS, 1>(p, a, stream)
-                               : launch_attention_t<DC, HD, DK, DV, KV, KVS, 0>(p, a, stream);
+template <int DC, int HD, int DK, int DV, int KV, int KVS, bool IP>
+static int launch_attention(const sfb_attn_params* p, const sfb_attn_ip_params* ipp, const AttnArgs& a,
+                            cudaStream_t stream) {
+    return a.dtype == SFB_BF16 ? launch_attention_t<DC, HD, DK, DV, KV, KVS, 1, IP>(p, ipp, a, stream)
+                               : launch_attention_t<DC, HD, DK, DV, KV, KVS, 0, IP>(p, ipp, a, stream);
 }
 
-}  // namespace sfb
-
-using namespace sfb;
-
-extern "C" int sfb_attention(const sfb_attn_params* p, sfb_stream_t stream_) {
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// Argument checks and the (head_dim, kv_tile) dispatch both entry points share; `ipp` is non-null for the
+// image-prompt variant only (checked by the caller).
+template <bool IP>
+static int attention_dispatch(const sfb_attn_params* p, const sfb_attn_ip_params* ipp, cudaStream_t stream) {
+    const char* what = IP ? "sfb_attention_ip" : "sfb_attention";
     if (!p || !p->tmap_q || !p->tmap_k || !p->tmap_vt || !p->out)
-        return fail(SFB_ERR_INVALID, "sfb_attention: null argument");
+        return fail(SFB_ERR_INVALID, "%s: null argument", what);
     if (p->head_dim % 8 || p->head_dim <= 0 || p->seq_q <= 0 || p->seq_kv <= 0)
-        return fail(SFB_ERR_INVALID, "sfb_attention: bad geometry");
+        return fail(SFB_ERR_INVALID, "%s: bad geometry", what);
     // V^T carries one extra all-ones row at index head_dim (softmax denominator on the tensor
     // core), so its row count is (head_dim + 1) rounded up to 16
     const int dv = (p->head_dim + 1 + 15) / 16 * 16;
     if (p->vt_rows != dv)
-        return fail(SFB_ERR_INVALID, "sfb_attention: vt_rows=%d must be (head_dim+1) rounded to 16 (%d)", p->vt_rows, dv);
+        return fail(SFB_ERR_INVALID, "%s: vt_rows=%d must be (head_dim+1) rounded to 16 (%d)", what, p->vt_rows, dv);
     AttnArgs a{};
     a.out = p->out; a.batch = p->batch; a.heads = p->heads; a.head_dim = p->head_dim;
     a.seq_q = p->seq_q; a.seq_kv = p->seq_kv; a.q_rows = p->q_rows; a.k_rows = p->k_rows;
@@ -345,26 +487,48 @@ extern "C" int sfb_attention(const sfb_attn_params* p, sfb_stream_t stream_) {
     a.scale_log2 = p->scale * 1.4426950408889634f;
     a.causal = p->causal ? 1 : 0;
     if (a.causal && (p->kv_tile != 64 || p->seq_q != p->seq_kv))
-        return fail(SFB_ERR_INVALID, "sfb_attention: causal needs kv_tile 64 and seq_q == seq_kv");
+        return fail(SFB_ERR_INVALID, "%s: causal needs kv_tile 64 and seq_q == seq_kv", what);
     if (p->kv_tile == 64) {  // v2: the caller built tmap_k with a 64-row box
         switch (p->head_dim) {
-            case 32: return launch_attention<1, 32, 32, 48, 64, 4>(p, a, stream);
-            case 40: return launch_attention<1, 40, 48, 48, 64, 4>(p, a, stream);
-            case 64: return launch_attention<1, 64, 64, 80, 64, 3>(p, a, stream);
-            case 160: return launch_attention<3, 160, 160, 176, 64, 2>(p, a, stream);
+            case 32: return launch_attention<1, 32, 32, 48, 64, 4, IP>(p, ipp, a, stream);
+            case 40: return launch_attention<1, 40, 48, 48, 64, 4, IP>(p, ipp, a, stream);
+            case 64: return launch_attention<1, 64, 64, 80, 64, 3, IP>(p, ipp, a, stream);
+            case 160: return launch_attention<3, 160, 160, 176, 64, 2, IP>(p, ipp, a, stream);
             default:
-                return fail(SFB_ERR_INVALID, "sfb_attention: kv_tile 64 supports head_dim 32 / 40 / 64 / 160, not %d", p->head_dim);
+                return fail(SFB_ERR_INVALID, "%s: kv_tile 64 supports head_dim 32 / 40 / 64 / 160, not %d", what,
+                            p->head_dim);
         }
     }
-    if (p->kv_tile != 0 && p->kv_tile != 128) return fail(SFB_ERR_INVALID, "sfb_attention: kv_tile must be 0, 64 or 128");
+    if (p->kv_tile != 0 && p->kv_tile != 128) return fail(SFB_ERR_INVALID, "%s: kv_tile must be 0, 64 or 128", what);
     switch (p->head_dim) {
-        case 32: return launch_attention<1, 32, 32, 48, 128, 2>(p, a, stream);
-        case 40: return launch_attention<1, 40, 48, 48, 128, 2>(p, a, stream);
-        case 64: return launch_attention<1, 64, 64, 80, 128, 2>(p, a, stream);
-        case 80: return launch_attention<2, 80, 80, 96, 128, 2>(p, a, stream);
-        case 128: return launch_attention<2, 128, 128, 144, 128, 1>(p, a, stream);
-        case 160: return launch_attention<3, 160, 160, 176, 128, 1>(p, a, stream);
+        case 32: return launch_attention<1, 32, 32, 48, 128, 2, IP>(p, ipp, a, stream);
+        case 40: return launch_attention<1, 40, 48, 48, 128, 2, IP>(p, ipp, a, stream);
+        case 64: return launch_attention<1, 64, 64, 80, 128, 2, IP>(p, ipp, a, stream);
+        case 80: return launch_attention<2, 80, 80, 96, 128, 2, IP>(p, ipp, a, stream);
+        case 128: return launch_attention<2, 128, 128, 144, 128, 1, IP>(p, ipp, a, stream);
+        case 160: return launch_attention<3, 160, 160, 176, 128, 1, IP>(p, ipp, a, stream);
         default:
-            return fail(SFB_ERR_INVALID, "sfb_attention: unsupported head_dim %d", p->head_dim);
+            return fail(SFB_ERR_INVALID, "%s: unsupported head_dim %d", what, p->head_dim);
     }
+}
+
+}  // namespace sfb
+
+using namespace sfb;
+
+extern "C" int sfb_attention(const sfb_attn_params* p, sfb_stream_t stream) {
+    return attention_dispatch<false>(p, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int sfb_attention_ip(const sfb_attn_ip_params* p, sfb_stream_t stream) {
+    if (!p || !p->tmap_k_ip || !p->tmap_vt_ip || !p->ip_scale)
+        return fail(SFB_ERR_INVALID, "sfb_attention_ip: null argument (tmap_k_ip / tmap_vt_ip / ip_scale)");
+    const int kv = p->base.kv_tile == 64 ? 64 : 128;
+    if (p->seq_ip <= 0 || p->seq_ip > kv)
+        return fail(SFB_ERR_INVALID, "sfb_attention_ip: seq_ip=%d must be in 1..kv_tile (%d): the image tokens are "
+                    "one KV tile", p->seq_ip, kv);
+    if (p->k_ip_rows < p->seq_ip)
+        return fail(SFB_ERR_INVALID, "sfb_attention_ip: k_ip_rows=%d < seq_ip=%d", p->k_ip_rows, p->seq_ip);
+    if (p->base.causal) return fail(SFB_ERR_INVALID, "sfb_attention_ip: causal is not supported");
+    return attention_dispatch<true>(&p->base, p, static_cast<cudaStream_t>(stream));
 }

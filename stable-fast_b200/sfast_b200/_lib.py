@@ -54,6 +54,13 @@ class AttnParams(C.Structure):
     ]
 
 
+class AttnIpParams(C.Structure):
+    _fields_ = [
+        ("base", AttnParams), ("tmap_k_ip", C.c_void_p), ("tmap_vt_ip", C.c_void_p),
+        ("seq_ip", C.c_int32), ("k_ip_rows", C.c_int32), ("ip_scale", C.c_void_p),
+    ]
+
+
 class GnParams(C.Structure):
     _fields_ = [
         ("x", C.c_void_p), ("y", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p),
@@ -138,6 +145,7 @@ SYMBOLS = {
     "sfb_tmap_nhwc": (C.c_int, [_VP, _VP, _U32, _U32, _U32, _U32, _U64, _U32, _U32, _U32, _U32]),
     "sfb_gemm": (C.c_int, [C.POINTER(GemmParams), _VP]),
     "sfb_attention": (C.c_int, [C.POINTER(AttnParams), _VP]),
+    "sfb_attention_ip": (C.c_int, [C.POINTER(AttnIpParams), _VP]),
     "sfb_group_norm_stats": (C.c_int, [C.POINTER(GnParams), _VP]),
     "sfb_group_norm_apply": (C.c_int, [C.POINTER(GnParams), _VP]),
     "sfb_group_norm_scale_shift": (C.c_int, [C.POINTER(GnParams), _VP, _VP]),

@@ -311,7 +311,14 @@ def attention_kv_tile(head_dim):
 
 
 def attention_op(name, lib, *, q, k, vt, out, batch, heads, head_dim, seq_q, seq_kv, q_rows, k_rows,
-                 vt_rows, q_pitch, vt_pitch, dt, dry=False, kv_tile=None, causal=False):
+                 vt_rows, q_pitch, vt_pitch, dt, dry=False, kv_tile=None, causal=False, ip=None):
+    """sfb_attention; with `ip` (dict: k, vt, seq, k_rows, vt_pitch, scale -- a one-float device tensor)
+    sfb_attention_ip, which adds scale * softmax(q k_ip^T / sqrt(D)) v_ip."""
+    if ip is not None:
+        return _attention_ip_op(name, lib, ip, attention_op(
+            name, lib, q=q, k=k, vt=vt, out=out, batch=batch, heads=heads, head_dim=head_dim, seq_q=seq_q,
+            seq_kv=seq_kv, q_rows=q_rows, k_rows=k_rows, vt_rows=vt_rows, q_pitch=q_pitch, vt_pitch=vt_pitch,
+            dt=dt, dry=dry, kv_tile=kv_tile), dry)
     bh = batch * heads
     # v2 kernel (64-key tiles, double-buffered score / probability tiles) for head_dim <= 64
     if kv_tile is None:
@@ -332,6 +339,28 @@ def attention_op(name, lib, *, q, k, vt, out, batch, heads, head_dim, seq_q, seq
     flops = 4 * batch * heads * seq_q * seq_kv * head_dim
     nbytes = 2 * bh * (2 * seq_q + 2 * seq_kv) * head_dim
     return Op(name, lib.sfb_attention, (C.byref(p),), (p, tq, tk, tv, q, k, vt, out), flops, nbytes)
+
+
+def _attention_ip_op(name, lib, ip, text, dry):
+    """The sfb_attention_ip launch around the text attention op `text` (its params become `base`)."""
+    p0, tq, tk, tv = text.keep[:4]
+    bh = p0.batch * p0.heads
+    tki = matrix_map(_ptr(ip["k"]), bh * ip["k_rows"], tk_cols(p0.head_dim), tk_cols(p0.head_dim), p0.kv_tile, dry)
+    tvi = matrix_map(_ptr(ip["vt"]), bh * p0.vt_rows, ip["vt_pitch"], ip["vt_pitch"], p0.vt_rows, dry)
+    p = _lib.AttnIpParams()
+    p.base = p0
+    p.tmap_k_ip, p.tmap_vt_ip = tki.ptr, tvi.ptr
+    p.seq_ip, p.k_ip_rows = ip["seq"], ip["k_rows"]
+    p.ip_scale = _ptr(ip["scale"])
+    flops = text.flops + 4 * bh * p0.seq_q * ip["seq"] * p0.head_dim
+    nbytes = text.bytes + 2 * bh * 2 * ip["seq"] * p0.head_dim
+    return Op(name, lib.sfb_attention_ip, (C.byref(p),),
+              (p, tki, tvi, ip["k"], ip["vt"], ip["scale"]) + tuple(text.keep[1:]), flops, nbytes)
+
+
+def tk_cols(head_dim):
+    """Element pitch of a Q / K row: head_dim rounded up to 64 (one 128-byte swizzle row per 64 dims)."""
+    return (head_dim + 63) // 64 * 64
 
 
 def gn_fused_fits(n, hw, c, groups):

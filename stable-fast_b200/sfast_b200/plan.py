@@ -600,7 +600,9 @@ class Plan:
 class UNetPlan(Plan):
     """One static launch schedule of the UNet for a fixed (batch, height, width)."""
 
-    def __init__(self, weights: PackedWeights, batch, height, width, ctx_len=77, controlnet=False):
+    def __init__(self, weights: PackedWeights, batch, height, width, ctx_len=77, controlnet=False, ip_len=0):
+        """`ip_len` > 0: an IP-Adapter (spec.ip) adds ip_len image tokens per sample (n_img images x its
+        tokens per image) to every cross-attention; 0 builds exactly the schedule without one."""
         spec = weights.spec
         div = 1 << (len(spec.block_out_channels) - 1)
         if height % div or width % div:
@@ -623,6 +625,21 @@ class UNetPlan(Plan):
         if spec.addition_embed_type == "text_time":
             self.add_in = self._alloc((batch, spec.add_in_dim), self.dt)
             self.time_ids_in = self._alloc((batch * 6,), torch.float32)
+        self.ip_len = ip_len
+        if ip_len:
+            ip = spec.ip
+            if ip is None or ip_len % ip.tokens:
+                raise ValueError(f"ip_len={ip_len} needs an IP-Adapter spec with a multiple of its tokens per image")
+            kv = min(ops.attention_kv_tile(t.head_dim) for _, t in spec.cross_attention_layers())
+            if ip_len > kv:
+                raise NotImplementedError(f"sfast (H100 build): {ip_len} IP-Adapter image tokens per sample; the "
+                                          f"fused attention takes at most {kv} (one KV tile)")
+            # static inputs: the image embeddings [B * n_img, D_img] and one scale per cross-attention (device
+            # memory: a captured graph serves every scale, per-block scales included)
+            self.image_embeds_in = self._alloc((batch * (ip_len // ip.tokens), ip.image_embed_dim), self.dt)
+            self.ip_scale_in = self._alloc((len(ip.layers),), torch.float32)
+            self._ip_slot = {p: i for i, p in enumerate(ip.layers)}
+            self._ip_tokens = None
         self._build()
 
     @staticmethod
@@ -707,9 +724,48 @@ class UNetPlan(Plan):
                 self._joined = True
                 self._emit(_JoinOp("all"))
         ao = self.act("attn_out", hs.n, hs.h, hs.w, C)
+        if cross and self.ip_len:
+            self.attention_core(a + ".core", qkv, ao, ip=self._ip_kv(a, B, t))
+            return self.linear(a + ".to_out", ao, self.w.matrix(f"{a}.to_out.0.weight"),
+                               self.w.f32(f"{a}.to_out.0.bias"), hs, residual=hs, rowstats_out=stats_next)
         self.attention_core(a + ".core", qkv, ao)
         self.linear(a + ".to_out", ao, self.w.matrix(f"{a}.to_out.0.weight"),
                     self.w.f32(f"{a}.to_out.0.bias"), hs, residual=hs, rowstats_out=stats_next)
+
+    def _ip_kv(self, a, B, t):
+        """IP-Adapter operands of cross-attention `a` (side stream, before the join of the first one): the
+        image tokens LayerNorm(image_embeds W^T + b) once per step, then this layer's K / V^T of them through
+        the QKV-scatter epilogue into its own buffers.  Returns the `ip` argument of ops.attention_op."""
+        ip, lib = self.spec.ip, self.lib_or_dry()
+        if self._ip_tokens is None:
+            pp = "encoder_hid_proj.image_projection_layers.0"
+            rows = self.image_embeds_in.shape[0]
+            proj = self.buf("ip_proj", (rows, ip.tokens * ip.ctx_dim))
+            self.side_ops.append(ops.small_linear_op(
+                pp + ".image_embeds", lib, x=self.image_embeds_in, w=self.w.small(pp + ".image_embeds.weight"),
+                bias=self.w.f32(pp + ".image_embeds.bias"), batch=rows, n=ip.tokens * ip.ctx_dim,
+                k=ip.image_embed_dim, dt=self.dt, y16=proj))
+            self._ip_tokens = self.buf("ip_tokens", (rows * ip.tokens, ip.ctx_dim))
+            self.side_ops.append(ops.ln_op(pp + ".norm", lib, x=proj, y=self._ip_tokens, rows=rows * ip.tokens,
+                                           c=ip.ctx_dim, gamma=self.w.f32(pp + ".norm.weight"),
+                                           beta=self.w.f32(pp + ".norm.bias"), eps=ip.norm_eps, dt=self.dt))
+        H, D, C = t.heads, t.head_dim, t.dim
+        kv_tile = ops.attention_kv_tile(D)
+        # k [B*H*ip_len, q_pitch] like the text K; v^T [B*H*dv, kv_tile]: one whole KV tile of columns, so the
+        # kernel's V^T loads stay inside the buffer (columns >= ip_len stay zero); no ones row is needed
+        dv, q_pitch = _round_up(D + 1, 16), _round_up(D, 64)
+        k = self.buf("attn_k_ip@" + a, (B * H * self.ip_len, q_pitch))
+        vt = self.buf("attn_vt_ip@" + a, (B * H * dv, kv_tile))
+        wkv = self.w.cat_matrix([f"{a}.processor.to_k_ip.0.weight", f"{a}.processor.to_v_ip.0.weight"])
+        tok = Act(self._ip_tokens, B, 1, self.ip_len, ip.ctx_dim)
+        self.side_ops.append(self._gemm(
+            a + ".ip_kv", a=self._a_matrix(tok), b=wkv, M=tok.rows, N=2 * C, K=ip.ctx_dim, dt=self.dt, epi=EPI_QKV,
+            qkv=dict(k=k, vt=vt, heads=H, head_dim=D, which_base=1, seq=self.ip_len, q_pitch=q_pitch,
+                     q_rows=self.ip_len, k_rows=self.ip_len, vt_rows=dv, vt_pitch=kv_tile),
+            splits=1, keep=(self._ip_tokens, wkv)))
+        i = self._ip_slot[a]
+        return dict(k=k, vt=vt, seq=self.ip_len, k_rows=self.ip_len, vt_pitch=kv_tile,
+                    scale=self.ip_scale_in[i:i + 1])
 
     def transformer(self, t, x: Act, dst: Act):
         p = t.prefix

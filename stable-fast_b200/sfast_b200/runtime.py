@@ -16,7 +16,7 @@ import torch
 
 from .plan import PackedWeights, UNetPlan
 from .svd_plan import SVDPlan
-from .unet_spec import cfg_get, spec_from_config
+from .unet_spec import cfg_get, ip_adapter_spec, ip_scale_of, spec_from_config
 
 logger = logging.getLogger(__name__)
 
@@ -163,9 +163,51 @@ class CompiledUNet(_CompiledModule):
 
     _what = "UNet"
 
-    def __init__(self, config, state_dict_fn, enable_cuda_graph=True, preserve_parameters=True):
+    def __init__(self, config, state_dict_fn, enable_cuda_graph=True, preserve_parameters=True, module=None):
+        """`module`: the UNet itself.  It is where a loaded IP-Adapter lives (``encoder_hid_proj`` and the
+        cross-attention processors, whose ``scale`` is read on every call); without it no adapter can be
+        compiled."""
         super().__init__(spec_from_config(config), state_dict_fn, enable_cuda_graph, preserve_parameters)
         self.first_call_s = None  # wall time of the first call (packing + plan + capture)
+        self._module = module
+        self._ip_proj = getattr(module, "encoder_hid_proj", None)
+        self._ip_procs = None
+        if cfg_get(config, "encoder_hid_dim_type") == "ip_image_proj" or self._ip_proj is not None:
+            if module is None:
+                raise NotImplementedError("sfast (H100 build): an IP-Adapter UNet is compiled from the module "
+                                          "(compile_unet_module), not from its config alone")
+            self.spec.ip = ip_adapter_spec(module, self.spec)
+            self._ip_procs = [module.get_submodule(p).processor for p in self.spec.ip.layers]
+
+    def _ip_inputs(self, added_cond_kwargs, cross_attention_kwargs, B):
+        """(ip_len, image embeddings [B * n_img, D_img], per-layer scales) of this call; (0, None, None) without
+        an adapter.  Refuses, by name, what the fused attention does not compute."""
+        if cross_attention_kwargs and "ip_adapter_masks" in cross_attention_kwargs:
+            raise NotImplementedError("sfast (H100 build): cross_attention_kwargs['ip_adapter_masks'] (IP-Adapter "
+                                      "masks) is not supported by the H100 path")
+        if self._module is not None and getattr(self._module, "encoder_hid_proj", None) is not self._ip_proj:
+            raise NotImplementedError("sfast (H100 build): the UNet's IP-Adapter was loaded, unloaded or replaced "
+                                      "after compile(); call compile() again")
+        ip = self.spec.ip
+        if ip is None:
+            return 0, None, None
+        if not added_cond_kwargs or "image_embeds" not in added_cond_kwargs:
+            raise ValueError(f"{type(self._module).__name__} has the config param `encoder_hid_dim_type` set to "
+                             "'ip_image_proj' which requires the keyword argument `image_embeds` to be passed in "
+                             "`added_cond_kwargs`")
+        emb = added_cond_kwargs["image_embeds"]
+        if isinstance(emb, (list, tuple)):
+            if len(emb) != 1:
+                raise NotImplementedError(f"sfast (H100 build): {len(emb)} image_embeds entries (one per "
+                                          "IP-Adapter); one adapter is supported")
+            emb = emb[0]
+        if emb.dim() == 2:  # diffusers' deprecated bare [B, D_img] form: one image per sample
+            emb = emb.unsqueeze(1)
+        if emb.dim() != 3 or emb.shape[0] != B or emb.shape[2] != ip.image_embed_dim:
+            raise ValueError(f"image_embeds of shape {tuple(emb.shape)}: expected [{B}, n_images, "
+                             f"{ip.image_embed_dim}]")
+        scales = [ip_scale_of(p, n) for p, n in zip(self._ip_procs, ip.layers)]
+        return emb.shape[1] * ip.tokens, emb.reshape(-1, ip.image_embed_dim), scales
 
     # -- forward -------------------------------------------------------------------------
     def _call_svd(self, sample, timestep, encoder_hidden_states, added_time_ids, return_dict=True):
@@ -219,6 +261,8 @@ class CompiledUNet(_CompiledModule):
         for k in _UNSUPPORTED_KWARGS:
             if given[k] is not None:
                 raise NotImplementedError(f"sfast (H100 build): UNet argument `{k}` is not supported")
+        B, _, H, W = sample.shape
+        ip_len, image_embeds, ip_scales = self._ip_inputs(added_cond_kwargs, cross_attention_kwargs, B)
         if cross_attention_kwargs:
             scale = cross_attention_kwargs.get("scale", 1.0)
             if set(cross_attention_kwargs) - {"scale"} or scale != 1.0:
@@ -228,7 +272,6 @@ class CompiledUNet(_CompiledModule):
         dtype = sample.dtype
         if dtype not in (torch.float16, torch.bfloat16):
             raise NotImplementedError(f"sfast (H100 build): UNet dtype {dtype}; use fp16 or bf16")
-        B, _, H, W = sample.shape
         ctx_len = encoder_hidden_states.shape[1]
         controlnet = down_block_additional_residuals is not None or mid_block_additional_residual is not None
         if controlnet and (down_block_additional_residuals is None or mid_block_additional_residual is None):
@@ -238,9 +281,12 @@ class CompiledUNet(_CompiledModule):
         with self._lock, torch.cuda.device(sample.device):
             t_first = time.perf_counter() if self.first_call_s is None else None
             weights = self._weights_for(dtype, sample.device)
-            gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index, controlnet),
-                               lambda: UNetPlan(weights, B, H, W, ctx_len, controlnet=controlnet))
+            gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index, controlnet, ip_len),
+                               lambda: UNetPlan(weights, B, H, W, ctx_len, controlnet=controlnet, ip_len=ip_len))
             plan = gp.plan
+            if ip_len:
+                plan.image_embeds_in.copy_(image_embeds, non_blocking=True)
+                plan.ip_scale_in.copy_(torch.tensor(ip_scales, dtype=torch.float32))
             plan.sample_in.copy_(sample, non_blocking=True)
             plan.ehs_in.copy_(encoder_hidden_states, non_blocking=True)
             t = timestep if torch.is_tensor(timestep) else torch.tensor(float(timestep))
@@ -698,7 +744,7 @@ def compile_controlnet_module(m, enable_cuda_graph=True, preserve_parameters=Tru
 def compile_unet_module(m, enable_cuda_graph=True, preserve_parameters=True):
     """Replace ``m.forward`` (same module object, as the reference does at
     /root/reference/src/sfast/compilers/diffusion_pipeline_compiler.py:146-149)."""
-    compiled = CompiledUNet(m.config, m.state_dict, enable_cuda_graph, preserve_parameters)
+    compiled = CompiledUNet(m.config, m.state_dict, enable_cuda_graph, preserve_parameters, module=m)
 
     def forward(*args, **kwargs):
         return compiled(*args, **kwargs)

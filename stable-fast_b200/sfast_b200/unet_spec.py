@@ -67,6 +67,19 @@ class BlockSpec:
 
 
 @dataclass
+class IPAdapterSpec:
+    """Geometry of one plain IP-Adapter (diffusers ``ImageProjection`` + ``IPAdapterAttnProcessor2_0``):
+    image embeddings of `image_embed_dim` are projected to `tokens` context tokens of `ctx_dim` each
+    (linear, then LayerNorm with `norm_eps`); every cross-attention in `layers` (attn2 prefixes, in
+    schedule order) attends to them with its own K / V projections and a scale read per call."""
+    image_embed_dim: int
+    tokens: int
+    ctx_dim: int
+    layers: tuple
+    norm_eps: float = 1e-5
+
+
+@dataclass
 class UNetSpec:
     in_channels: int
     out_channels: int
@@ -89,6 +102,7 @@ class UNetSpec:
     cond_channels: int = 0
     cond_embed_channels: tuple = ()
     cond_bgr: bool = False
+    ip: Optional[IPAdapterSpec] = None  # an IP-Adapter is loaded (UNet only)
 
     @property
     def temporal(self):
@@ -103,6 +117,12 @@ class UNetSpec:
                 if r.temporal_prefix:
                     out.append(ResnetSpec(r.temporal_prefix, r.cout, r.cout, r.eps))
         return out
+
+    def cross_attention_layers(self):
+        """(attn2 prefix, TransformerSpec) of every cross-attention, in the order the plan runs them."""
+        return [(f"{t.prefix}.transformer_blocks.{d}.attn2", t)
+                for b in self.down + [self.mid] + self.up for t in b.attentions if t is not None
+                for d in range(t.depth)]
 
     def residual_channels(self):
         """Channels of the ControlNet's down-block residuals, in diffusers' order: conv_in's output, then
@@ -120,7 +140,9 @@ _SUPPORTED_UP = ("CrossAttnUpBlock2D", "UpBlock2D")
 def spec_from_config(cfg) -> UNetSpec:
     if is_svd_config(cfg):
         return svd_spec_from_config(cfg)
-    spec, tf, layers = _encoder_spec(cfg, out_channels=cfg_get(cfg, "out_channels", 4))
+    # an IP-Adapter sets encoder_hid_dim_type = "ip_image_proj"; its geometry is read from the module
+    # (ip_adapter_spec), not the config.  A ControlNet never receives image embeddings: it keeps refusing it.
+    spec, tf, layers = _encoder_spec(cfg, out_channels=cfg_get(cfg, "out_channels", 4), accept_ip=True)
     up_types = tuple(cfg_get(cfg, "up_block_types"))
     for t in up_types:
         if t not in _SUPPORTED_UP:
@@ -145,10 +167,11 @@ def spec_from_config(cfg) -> UNetSpec:
     return spec
 
 
-def _encoder_spec(cfg, out_channels):
+def _encoder_spec(cfg, out_channels, accept_ip=False):
     """The part of the architecture a UNet and a ControlNet share (time embedding, conv_in, down blocks,
     mid block), with every check of the config keys both carry.  Returns (spec without up blocks, the
-    transformer-spec factory, layers per block)."""
+    transformer-spec factory, layers per block).  `accept_ip`: encoder_hid_dim_type="ip_image_proj" (an
+    IP-Adapter) passes; the caller reads the adapter from the module."""
     boc = tuple(cfg_get(cfg, "block_out_channels"))
     nb = len(boc)
     down_types = tuple(cfg_get(cfg, "down_block_types"))
@@ -159,6 +182,8 @@ def _encoder_spec(cfg, out_channels):
                 "resnet_time_scale_shift", "dual_cross_attention", "only_cross_attention",
                 "upcast_attention", "time_embedding_act_fn", "attention_type"):
         v = cfg_get(cfg, key)
+        if accept_ip and key == "encoder_hid_dim_type" and v == "ip_image_proj":
+            continue
         if v not in (None, False, "default", "positional"):
             raise NotImplementedError(f"UNet config {key}={v!r} is not supported by the H100 path")
     # fields whose only supported value is the SD-1.5 / SDXL one: anything else would compile and
@@ -251,6 +276,79 @@ def controlnet_spec_from_config(cfg) -> UNetSpec:
     spec, _, _ = _encoder_spec(cfg, out_channels=0)
     spec.cond_channels, spec.cond_embed_channels, spec.cond_bgr = cc, emb, order == "bgr"
     return spec
+
+
+def ip_adapter_geometry(spec: UNetSpec, image_embed_dim, tokens=4, norm_eps=1e-5) -> IPAdapterSpec:
+    """The IPAdapterSpec of a plain IP-Adapter on `spec`'s UNet (every cross-attention carries it)."""
+    return IPAdapterSpec(int(image_embed_dim), int(tokens), spec.cross_attention_dim,
+                         tuple(p for p, _ in spec.cross_attention_layers()), float(norm_eps))
+
+
+_FACEID_PROJECTIONS = ("IPAdapterFaceIDImageProjection", "IPAdapterFaceIDPlusImageProjection")
+
+
+def ip_adapter_spec(unet, spec: UNetSpec) -> IPAdapterSpec:
+    """Read the IP-Adapter loaded on a diffusers UNet (``pipe.load_ip_adapter``): exactly one
+    ``ImageProjection`` in ``unet.encoder_hid_proj`` and, on every cross-attention, an
+    ``IPAdapterAttnProcessor2_0``-like ``processor`` with ``to_k_ip[0]`` / ``to_v_ip[0]`` and a one-float
+    ``scale``.  Anything else is refused by name: it would otherwise compute something different."""
+    def refuse(what):
+        raise NotImplementedError(f"sfast (H100 build): {what} is not supported by the H100 path (one plain "
+                                  "IP-Adapter with an ImageProjection is)")
+    if getattr(unet, "text_encoder_hid_proj", None) is not None:
+        refuse("text_encoder_hid_proj (a text projection next to the IP-Adapter)")
+    proj = getattr(unet, "encoder_hid_proj", None)
+    if proj is None:
+        refuse("encoder_hid_dim_type='ip_image_proj' without an encoder_hid_proj")
+    layers = getattr(proj, "image_projection_layers", None)
+    if layers is None:
+        refuse(f"encoder_hid_proj of type {type(proj).__name__}")
+    layers = list(layers)
+    if len(layers) != 1:
+        refuse(f"more than one IP-Adapter at once ({len(layers)} image projections)")
+    lay = layers[0]
+    kind = type(lay).__name__
+    if kind == "IPAdapterPlusImageProjection":
+        refuse("IPAdapterPlusImageProjection (IP-Adapter Plus, Resampler)")
+    if kind in _FACEID_PROJECTIONS:
+        refuse(f"{kind} (IP-Adapter FaceID)")
+    if kind != "ImageProjection":
+        refuse(f"image projection {kind}")
+    lin, norm = lay.image_embeds, lay.norm
+    tokens = int(getattr(lay, "num_image_text_embeds", 0) or 0)
+    ctx = int(getattr(lay, "cross_attention_dim", norm.normalized_shape[0]))
+    if ctx != spec.cross_attention_dim or tuple(norm.normalized_shape) != (ctx,) or \
+            tokens <= 0 or lin.out_features != tokens * ctx:
+        refuse(f"ImageProjection geometry (tokens {tokens}, context {ctx}, linear {lin.out_features}, UNet "
+               f"cross_attention_dim {spec.cross_attention_dim})")
+    ip = ip_adapter_geometry(spec, lin.in_features, tokens, norm.eps)
+    dims = dict(spec.cross_attention_layers())
+    for prefix in ip.layers:
+        proc = getattr(unet.get_submodule(prefix), "processor", None)
+        k, v = getattr(proc, "to_k_ip", None), getattr(proc, "to_v_ip", None)
+        if k is None or v is None:
+            refuse(f"{prefix}.processor of type {type(proc).__name__} (no to_k_ip / to_v_ip)")
+        if len(k) != 1 or len(v) != 1:
+            refuse(f"more than one IP-Adapter at once ({prefix}.processor has {len(k)} image K projections)")
+        C = dims[prefix].dim
+        for lin_ in (k[0], v[0]):
+            if tuple(lin_.weight.shape) != (C, ctx) or getattr(lin_, "bias", None) is not None:
+                refuse(f"{prefix}.processor image K/V projection of shape {tuple(lin_.weight.shape)}")
+        ip_scale_of(proc, prefix)
+    return ip
+
+
+def ip_scale_of(proc, prefix):
+    """The one float an IPAdapterAttnProcessor2_0's `scale` holds (set_ip_adapter_scale writes it in place)."""
+    scale = getattr(proc, "scale", None)
+    if not isinstance(scale, (list, tuple)) or len(scale) != 1:
+        raise NotImplementedError(f"sfast (H100 build): {prefix}.processor.scale={scale!r} is not supported by "
+                                  "the H100 path (one float per layer)")
+    s = scale[0]
+    if isinstance(s, (list, tuple)) or (torch.is_tensor(s) and s.numel() != 1):
+        raise NotImplementedError(f"sfast (H100 build): per-image IP-Adapter scale lists ({prefix}.processor."
+                                  f"scale={scale!r}) are not supported by the H100 path")
+    return float(s)
 
 
 _SVD_DOWN = ("CrossAttnDownBlockSpatioTemporal", "DownBlockSpatioTemporal")
@@ -452,6 +550,15 @@ def param_shapes(spec: UNetSpec):
         return out
     norm("conv_norm_out", spec.block_out_channels[0])
     conv("conv_out", spec.out_channels, spec.block_out_channels[0], 3)
+    if spec.ip is not None:
+        # diffusers' names after load_ip_adapter
+        ip, pp = spec.ip, "encoder_hid_proj.image_projection_layers.0"
+        lin(pp + ".image_embeds", ip.tokens * ip.ctx_dim, ip.image_embed_dim)
+        norm(pp + ".norm", ip.ctx_dim)
+        dims = dict(spec.cross_attention_layers())
+        for prefix in ip.layers:
+            lin(prefix + ".processor.to_k_ip.0", dims[prefix].dim, ip.ctx_dim, False)
+            lin(prefix + ".processor.to_v_ip.0", dims[prefix].dim, ip.ctx_dim, False)
     return out
 
 

@@ -52,7 +52,8 @@ def compile(m, config):
     """Compile a diffusers pipeline in place and return it (reference `compile`, :81-124): the UNet, the
     ControlNet (``pipe.controlnet``: a ControlNetModel, or each net of a MultiControlNetModel), the VAE, the
     text encoders and the image encoder run on the native path; a ControlNet class or config the native
-    path does not cover stays eager with a warning."""
+    path does not cover stays eager with a warning.  A loaded IP-Adapter (one plain ``ImageProjection`` or one
+    IP-Adapter Plus ``IPAdapterPlusImageProjection``) runs inside the UNet's step, see `compile_unet`."""
     m.unet = compile_unet(m.unet, config)
     if getattr(m, 'controlnet', None) is not None:
         m.controlnet = compile_controlnet(m.controlnet, config)
@@ -134,7 +135,11 @@ def _compile_controlnet_net(m, config):
 def compile_unet(m, config):
     """Replace ``m.forward`` with the H100-native UNet step (reference `compile_unet`, :127-151).
 
-    There is no CPU / eager fallback: the module must live on an sm_90 CUDA device."""
+    There is no CPU / eager fallback: the module must live on an sm_90 CUDA device.  A loaded IP-Adapter is
+    compiled with it: a plain adapter's image projection, or IP-Adapter Plus's Resampler (its perceiver blocks
+    over the image features of ``added_cond_kwargs["image_embeds"]``, ``[B, n_img, S_img, D_img]``), runs on
+    the step's side stream inside the same CUDA graph, and every cross-attention adds the image-token term.
+    FaceID projections, several adapters and ``ip_adapter_masks`` raise ``NotImplementedError`` by name."""
     from sfast_b200.runtime import compile_unet_module, require_sm90
     device = m.device if hasattr(m, 'device') else torch.device(
         'cuda' if torch.cuda.is_available() else 'cpu')

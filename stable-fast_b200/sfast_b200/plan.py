@@ -16,6 +16,7 @@ Design points (see DESIGN.md):
     graph: time-embedding chain, cross-attention K/V projections, resnet shortcut GEMMs.
   * a split-K conv followed by a GroupNorm leaves its reduction to that GroupNorm kernel.
 """
+import ctypes as C
 import math
 import os
 
@@ -23,7 +24,7 @@ import torch
 
 from . import _lib, ops
 from .ops import Act, EPI_GEGLU, EPI_QKV, Op, _ptr
-from .unet_spec import UNetSpec, spec_from_config
+from .unet_spec import RESAMPLER_HEAD_DIM, UNetSpec, spec_from_config
 
 
 def _round_up(a, b):
@@ -510,15 +511,16 @@ class Plan:
                              eps=eps, dt=self.dt))
         return y
 
-    def attention_operands(self, B, H, S, skv, D, kv_tag=""):
+    def attention_operands(self, B, H, S, skv, D, kv_tag="", q_tag=""):
         """q [B*H*S, q_pitch], k [B*H*skv, q_pitch] and v^T [B*H*dv, vt_pitch] buffers of one flash-attention
         launch, as the QKV-scatter epilogue and the attention kernel address them.  v^T carries an all-ones
         row after the D value rows: P times it is the softmax denominator, computed on the tensor core.
-        `kv_tag` keeps k / v^T apart from other launches of the same shape (the UNet's hoisted cross K/V)."""
+        `kv_tag` keeps k / v^T apart from other launches of the same shape (the UNet's hoisted cross K/V);
+        `q_tag` does the same for q (operands written on the side stream)."""
         dv = _round_up(D + 1, 16)
         q_pitch, vt_pitch = _round_up(D, 64), _round_up(skv, 64)
         tag = f"{B}x{H}x{S}x{skv}x{D}"
-        q = self.buf("attn_q_" + tag, (B * H * S, q_pitch))
+        q = self.buf("attn_q_" + tag + q_tag, (B * H * S, q_pitch))
         k = self.buf("attn_k_" + tag + kv_tag, (B * H * skv, q_pitch))
         new_vt = ("attn_vt_" + tag + kv_tag, (B * H * dv, vt_pitch), self.dt) not in self._bufs
         vt = self.buf("attn_vt_" + tag + kv_tag, (B * H * dv, vt_pitch))
@@ -600,9 +602,11 @@ class Plan:
 class UNetPlan(Plan):
     """One static launch schedule of the UNet for a fixed (batch, height, width)."""
 
-    def __init__(self, weights: PackedWeights, batch, height, width, ctx_len=77, controlnet=False, ip_len=0):
+    def __init__(self, weights: PackedWeights, batch, height, width, ctx_len=77, controlnet=False, ip_len=0,
+                 ip_seq=0):
         """`ip_len` > 0: an IP-Adapter (spec.ip) adds ip_len image tokens per sample (n_img images x its
-        tokens per image) to every cross-attention; 0 builds exactly the schedule without one."""
+        tokens per image) to every cross-attention; 0 builds exactly the schedule without one.  `ip_seq`:
+        feature tokens per image of an IP-Adapter Plus (spec.ip.resampler), the input of its Resampler."""
         spec = weights.spec
         div = 1 << (len(spec.block_out_channels) - 1)
         if height % div or width % div:
@@ -634,9 +638,17 @@ class UNetPlan(Plan):
             if ip_len > kv:
                 raise NotImplementedError(f"sfast (H100 build): {ip_len} IP-Adapter image tokens per sample; the "
                                           f"fused attention takes at most {kv} (one KV tile)")
-            # static inputs: the image embeddings [B * n_img, D_img] and one scale per cross-attention (device
-            # memory: a captured graph serves every scale, per-block scales included)
-            self.image_embeds_in = self._alloc((batch * (ip_len // ip.tokens), ip.image_embed_dim), self.dt)
+            # static inputs: the image embeddings [B * n_img, D_img] (Plus: the image features [B * n_img *
+            # ip_seq, D_img]) and one scale per cross-attention (device memory: a captured graph serves every
+            # scale, per-block scales included)
+            rows = batch * (ip_len // ip.tokens)
+            self.ip_seq = 0
+            if ip.resampler is not None:
+                if ip_seq <= 0:
+                    raise ValueError("an IP-Adapter Plus plan needs ip_seq > 0 (image feature tokens per image)")
+                self.ip_seq = ip_seq
+                rows *= ip_seq
+            self.image_embeds_in = self._alloc((rows, ip.image_embed_dim), self.dt)
             self.ip_scale_in = self._alloc((len(ip.layers),), torch.float32)
             self._ip_slot = {p: i for i, p in enumerate(ip.layers)}
             self._ip_tokens = None
@@ -734,9 +746,12 @@ class UNetPlan(Plan):
 
     def _ip_kv(self, a, B, t):
         """IP-Adapter operands of cross-attention `a` (side stream, before the join of the first one): the
-        image tokens LayerNorm(image_embeds W^T + b) once per step, then this layer's K / V^T of them through
-        the QKV-scatter epilogue into its own buffers.  Returns the `ip` argument of ops.attention_op."""
+        image tokens LayerNorm(image_embeds W^T + b) (IP-Adapter Plus: the Resampler, _resampler) once per
+        step, then this layer's K / V^T of them through the QKV-scatter epilogue into its own buffers.  Returns
+        the `ip` argument of ops.attention_op."""
         ip, lib = self.spec.ip, self.lib_or_dry()
+        if self._ip_tokens is None and ip.resampler is not None:
+            self._ip_tokens = self._resampler(lib)
         if self._ip_tokens is None:
             pp = "encoder_hid_proj.image_projection_layers.0"
             rows = self.image_embeds_in.shape[0]
@@ -766,6 +781,81 @@ class UNetPlan(Plan):
         i = self._ip_slot[a]
         return dict(k=k, vt=vt, seq=self.ip_len, k_rows=self.ip_len, vt_pitch=kv_tile,
                     scale=self.ip_scale_in[i:i + 1])
+
+    def _resampler(self, lib):
+        """IP-Adapter Plus's image projection (diffusers ``IPAdapterPlusImageProjection``), on the side stream:
+        the image tokens [N * Q, ctx] of the image features image_embeds_in [N * S, D_img], N = B * n_img,
+        Q learned queries (latents), S = ip_seq.  Per block:
+            kv = cat(ln1(latents), ln0(x))                     x = proj_in(image features)
+            latents += to_out(attention(to_q(ln1(latents)), to_k(kv), to_v(kv)))   dim_head 64, scale 1/8
+            latents += ff.2(gelu(ff.1(ff.0(latents))))
+        then LayerNorm(proj_out(latents)).  diffusers concatenates (ln0(x), ln1(latents)); softmax . V is a
+        sum over keys, so the order is free: the Q latent keys come first and the S feature keys start at a
+        Q-row offset of K and a Q-column offset of V^T (16-byte aligned for Q % 8 == 0).  The two segments
+        are two QKV-scatter GEMMs into one K / V^T pair.  The latents are broadcast to N rows as
+        0 + latents[m % Q] (sfb_row_broadcast_add).  Every GEMM here is split-K free: the split-K workspace
+        is shared with the main stream."""
+        ip, rs, dt = self.spec.ip, self.spec.ip.resampler, self.dt
+        pp = "encoder_hid_proj.image_projection_layers.0"
+        Q, S, Dh, H, D = ip.tokens, self.ip_seq, rs.dim, rs.heads, RESAMPLER_HEAD_DIM
+        N = self.image_embeds_in.shape[0] // S
+        side = self.side_ops
+
+        def gemm(name, x: Act, wm, dst: Act = None, **kw):
+            keep = (x.buf, wm) + ((dst.buf,) if dst is not None else ())
+            if dst is not None:
+                kw.update(out=dst.ptr, ldo=dst.ld)
+            side.append(self._gemm(name, a=self._a_matrix(x), b=wm, M=x.rows, N=wm.n, K=x.c, dt=dt, splits=1,
+                                   keep=keep, **kw))
+
+        def layer_norm(name, x: Act, y: Act, eps):
+            side.append(ops.ln_op(name, lib, x=x.buf, y=y.buf, rows=x.rows, c=x.c, gamma=self.w.f32(name + ".weight"),
+                                  beta=self.w.f32(name + ".bias"), eps=eps, dt=dt))
+
+        lat = Act(self.buf("rs_latents", (N * Q, Dh)), N, 1, Q, Dh)
+        zero = Act(self.buf("rs_zero", (N * Q, Dh)), N, 1, Q, Dh)  # never written
+        latents = self.w.small(pp + ".latents")
+        p = _lib.RowOpParams()
+        p.x, p.y, p.vec, p.ldv = zero.ptr, lat.ptr, _ptr(latents), Dh
+        p.rows, p.c, p.ldx, p.ldy, p.dtype = lat.rows, Dh, Dh, Dh, ops.dtype_code(dt)
+        p.mode, p.div, p.mod = _lib.ROW_IDX_DIV_MOD, 1, Q
+        side.append(Op(pp + ".latents", lib.sfb_row_broadcast_add, (C.byref(p),),
+                       (p, zero.buf, lat.buf, latents, None, None, None), 0, 3 * lat.rows * Dh * 2))
+        x = Act(self.buf("rs_x", (N * S, Dh)), N, 1, S, Dh)
+        gemm(pp + ".proj_in", Act(self.image_embeds_in, N, 1, S, ip.image_embed_dim),
+             self.w.matrix(pp + ".proj_in.weight"), x, bias=self.w.f32(pp + ".proj_in.bias"))
+        skv = Q + S
+        qkv = self.attention_operands(N, H, Q, skv, D, kv_tag="@resampler", q_tag="@resampler")
+        esz = qkv["q"].element_size()
+        img_kv = dict(qkv, k=_ptr(qkv["k"]) + Q * qkv["q_pitch"] * esz, vt=_ptr(qkv["vt"]) + Q * esz, which_base=1,
+                      seq=S)
+        xn = Act(self.buf("rs_ln0", (N * S, Dh)), N, 1, S, Dh)
+        ln = Act(self.buf("rs_ln1", (N * Q, Dh)), N, 1, Q, Dh)
+        ao = Act(self.buf("rs_attn", (N * Q, rs.inner)), N, 1, Q, rs.inner)
+        hid = Act(self.buf("rs_ff", (N * Q, rs.ff_dim)), N, 1, Q, rs.ff_dim)
+        for i in range(rs.depth):
+            b = f"{pp}.layers.{i}"
+            e0, e1, e2 = rs.block_eps[i]
+            layer_norm(b + ".ln0", x, xn, e0)
+            layer_norm(b + ".ln1", lat, ln, e1)
+            wq, wk, wv = (f"{b}.attn.{n}.weight" for n in ("to_q", "to_k", "to_v"))
+            gemm(b + ".attn.qkv", ln, self.w.cat_matrix([wq, wk, wv]), epi=EPI_QKV,
+                 qkv=dict(qkv, which_base=0, seq=Q))
+            gemm(b + ".attn.kv_image", xn, self.w.cat_matrix([wk, wv]), epi=EPI_QKV, qkv=img_kv)
+            side.append(ops.attention_op(b + ".attn.core", lib, out=ao.buf, batch=N, seq_q=Q, seq_kv=skv, dt=dt,
+                                         dry=self.dry, **qkv))
+            gemm(b + ".attn.to_out", ao, self.w.matrix(b + ".attn.to_out.0.weight"), lat,
+                 residual=lat.ptr, ldr=lat.ld)
+            layer_norm(b + ".ff.0", lat, ln, e2)
+            gemm(b + ".ff.1.net.0.proj", ln, self.w.matrix(b + ".ff.1.net.0.proj.weight"), hid, act=_lib.ACT_GELU)
+            gemm(b + ".ff.1.net.2", hid, self.w.matrix(b + ".ff.1.net.2.weight"), lat, residual=lat.ptr,
+                 ldr=lat.ld)
+        proj = Act(self.buf("ip_proj", (N * Q, ip.ctx_dim)), N, 1, Q, ip.ctx_dim)
+        gemm(pp + ".proj_out", lat, self.w.matrix(pp + ".proj_out.weight"), proj,
+             bias=self.w.f32(pp + ".proj_out.bias"))
+        tokens = Act(self.buf("ip_tokens", (N * Q, ip.ctx_dim)), N, 1, Q, ip.ctx_dim)
+        layer_norm(pp + ".norm_out", proj, tokens, ip.norm_eps)
+        return tokens.buf
 
     def transformer(self, t, x: Act, dst: Act):
         p = t.prefix

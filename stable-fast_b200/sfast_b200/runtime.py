@@ -180,8 +180,10 @@ class CompiledUNet(_CompiledModule):
             self._ip_procs = [module.get_submodule(p).processor for p in self.spec.ip.layers]
 
     def _ip_inputs(self, added_cond_kwargs, cross_attention_kwargs, B):
-        """(ip_len, image embeddings [B * n_img, D_img], per-layer scales) of this call; (0, None, None) without
-        an adapter.  Refuses, by name, what the fused attention does not compute."""
+        """(ip_len, ip_seq, image embeddings, per-layer scales) of this call; (0, 0, None, None) without an
+        adapter.  The embeddings are [B * n_img, D_img] for a plain adapter (ip_seq 0) and the image features
+        [B * n_img * ip_seq, D_img] for IP-Adapter Plus.  Refuses, by name, what the fused attention does not
+        compute."""
         if cross_attention_kwargs and "ip_adapter_masks" in cross_attention_kwargs:
             raise NotImplementedError("sfast (H100 build): cross_attention_kwargs['ip_adapter_masks'] (IP-Adapter "
                                       "masks) is not supported by the H100 path")
@@ -190,24 +192,36 @@ class CompiledUNet(_CompiledModule):
                                       "after compile(); call compile() again")
         ip = self.spec.ip
         if ip is None:
-            return 0, None, None
+            return 0, 0, None, None
         if not added_cond_kwargs or "image_embeds" not in added_cond_kwargs:
             raise ValueError(f"{type(self._module).__name__} has the config param `encoder_hid_dim_type` set to "
                              "'ip_image_proj' which requires the keyword argument `image_embeds` to be passed in "
                              "`added_cond_kwargs`")
         emb = added_cond_kwargs["image_embeds"]
-        if isinstance(emb, (list, tuple)):
+        bare = not isinstance(emb, (list, tuple))
+        if not bare:
             if len(emb) != 1:
                 raise NotImplementedError(f"sfast (H100 build): {len(emb)} image_embeds entries (one per "
                                           "IP-Adapter); one adapter is supported")
             emb = emb[0]
-        if emb.dim() == 2:  # diffusers' deprecated bare [B, D_img] form: one image per sample
-            emb = emb.unsqueeze(1)
-        if emb.dim() != 3 or emb.shape[0] != B or emb.shape[2] != ip.image_embed_dim:
-            raise ValueError(f"image_embeds of shape {tuple(emb.shape)}: expected [{B}, n_images, "
-                             f"{ip.image_embed_dim}]")
+        if ip.resampler is not None:
+            # IP-Adapter Plus: image features (the vision tower's hidden_states[-2]) [B, n_img, S_img, D_img]; the
+            # deprecated bare [B, S_img, D_img] form is one image per sample
+            if bare and emb.dim() == 3:
+                emb = emb.unsqueeze(1)
+            if emb.dim() != 4 or emb.shape[0] != B or emb.shape[3] != ip.image_embed_dim or emb.shape[2] < 1:
+                raise ValueError(f"image_embeds of shape {tuple(emb.shape)}: expected [{B}, n_images, S_img, "
+                                 f"{ip.image_embed_dim}] (IP-Adapter Plus image features)")
+            ip_seq = emb.shape[2]
+        else:
+            if emb.dim() == 2:  # diffusers' deprecated bare [B, D_img] form: one image per sample
+                emb = emb.unsqueeze(1)
+            if emb.dim() != 3 or emb.shape[0] != B or emb.shape[2] != ip.image_embed_dim:
+                raise ValueError(f"image_embeds of shape {tuple(emb.shape)}: expected [{B}, n_images, "
+                                 f"{ip.image_embed_dim}]")
+            ip_seq = 0
         scales = [ip_scale_of(p, n) for p, n in zip(self._ip_procs, ip.layers)]
-        return emb.shape[1] * ip.tokens, emb.reshape(-1, ip.image_embed_dim), scales
+        return emb.shape[1] * ip.tokens, ip_seq, emb.reshape(-1, ip.image_embed_dim), scales
 
     # -- forward -------------------------------------------------------------------------
     def _call_svd(self, sample, timestep, encoder_hidden_states, added_time_ids, return_dict=True):
@@ -262,7 +276,7 @@ class CompiledUNet(_CompiledModule):
             if given[k] is not None:
                 raise NotImplementedError(f"sfast (H100 build): UNet argument `{k}` is not supported")
         B, _, H, W = sample.shape
-        ip_len, image_embeds, ip_scales = self._ip_inputs(added_cond_kwargs, cross_attention_kwargs, B)
+        ip_len, ip_seq, image_embeds, ip_scales = self._ip_inputs(added_cond_kwargs, cross_attention_kwargs, B)
         if cross_attention_kwargs:
             scale = cross_attention_kwargs.get("scale", 1.0)
             if set(cross_attention_kwargs) - {"scale"} or scale != 1.0:
@@ -281,8 +295,9 @@ class CompiledUNet(_CompiledModule):
         with self._lock, torch.cuda.device(sample.device):
             t_first = time.perf_counter() if self.first_call_s is None else None
             weights = self._weights_for(dtype, sample.device)
-            gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index, controlnet, ip_len),
-                               lambda: UNetPlan(weights, B, H, W, ctx_len, controlnet=controlnet, ip_len=ip_len))
+            gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index, controlnet, ip_len, ip_seq),
+                               lambda: UNetPlan(weights, B, H, W, ctx_len, controlnet=controlnet, ip_len=ip_len,
+                                                ip_seq=ip_seq))
             plan = gp.plan
             if ip_len:
                 plan.image_embeds_in.copy_(image_embeds, non_blocking=True)

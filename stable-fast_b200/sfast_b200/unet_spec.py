@@ -67,16 +67,38 @@ class BlockSpec:
 
 
 @dataclass
+class ResamplerSpec:
+    """Geometry of IP-Adapter Plus's image projection (diffusers ``IPAdapterPlusImageProjection``, the
+    "Resampler"): `dim` = hidden width Dh, `heads` attention heads of 64 dims, `depth` blocks with a FeedForward
+    of `ff_dim`, and the eps of each block's LayerNorms as ((ln0, ln1, ff.0), ...).  The learned latents are
+    the IPAdapterSpec's `tokens` queries; norm_out's eps is the IPAdapterSpec's `norm_eps`."""
+    dim: int
+    heads: int
+    depth: int
+    ff_dim: int
+    block_eps: tuple
+
+    @property
+    def inner(self):
+        return self.heads * RESAMPLER_HEAD_DIM
+
+
+RESAMPLER_HEAD_DIM = 64
+
+
+@dataclass
 class IPAdapterSpec:
-    """Geometry of one plain IP-Adapter (diffusers ``ImageProjection`` + ``IPAdapterAttnProcessor2_0``):
-    image embeddings of `image_embed_dim` are projected to `tokens` context tokens of `ctx_dim` each
-    (linear, then LayerNorm with `norm_eps`); every cross-attention in `layers` (attn2 prefixes, in
+    """Geometry of one IP-Adapter (diffusers ``ImageProjection`` or ``IPAdapterPlusImageProjection`` +
+    ``IPAdapterAttnProcessor2_0``): image embeddings of `image_embed_dim` are projected to `tokens` context
+    tokens of `ctx_dim` each (plain: linear, then LayerNorm with `norm_eps`; Plus: the `resampler` over the
+    image's feature tokens, `tokens` learned queries); every cross-attention in `layers` (attn2 prefixes, in
     schedule order) attends to them with its own K / V projections and a scale read per call."""
     image_embed_dim: int
     tokens: int
     ctx_dim: int
     layers: tuple
     norm_eps: float = 1e-5
+    resampler: Optional[ResamplerSpec] = None  # IP-Adapter Plus
 
 
 @dataclass
@@ -284,17 +306,30 @@ def ip_adapter_geometry(spec: UNetSpec, image_embed_dim, tokens=4, norm_eps=1e-5
                          tuple(p for p, _ in spec.cross_attention_layers()), float(norm_eps))
 
 
+def ip_adapter_plus_geometry(spec: UNetSpec, image_embed_dim, dim, tokens=16, depth=4, ff_mult=4,
+                             eps=1e-5) -> IPAdapterSpec:
+    """The IPAdapterSpec of an IP-Adapter Plus on `spec`'s UNet: a Resampler of hidden width `dim` (dim / 64
+    heads) with `tokens` learned queries and `depth` blocks, every LayerNorm with `eps`."""
+    ip = ip_adapter_geometry(spec, image_embed_dim, tokens, eps)
+    ip.resampler = ResamplerSpec(int(dim), int(dim) // RESAMPLER_HEAD_DIM, int(depth), int(dim) * ff_mult,
+                                 ((float(eps),) * 3,) * depth)
+    return ip
+
+
 _FACEID_PROJECTIONS = ("IPAdapterFaceIDImageProjection", "IPAdapterFaceIDPlusImageProjection")
 
 
 def ip_adapter_spec(unet, spec: UNetSpec) -> IPAdapterSpec:
     """Read the IP-Adapter loaded on a diffusers UNet (``pipe.load_ip_adapter``): exactly one
-    ``ImageProjection`` in ``unet.encoder_hid_proj`` and, on every cross-attention, an
-    ``IPAdapterAttnProcessor2_0``-like ``processor`` with ``to_k_ip[0]`` / ``to_v_ip[0]`` and a one-float
-    ``scale``.  Anything else is refused by name: it would otherwise compute something different."""
+    ``ImageProjection`` or ``IPAdapterPlusImageProjection`` in ``unet.encoder_hid_proj`` and, on every
+    cross-attention, an ``IPAdapterAttnProcessor2_0``-like ``processor`` with ``to_k_ip[0]`` / ``to_v_ip[0]``
+    and a one-float ``scale``.  Anything else is refused by name: it would otherwise compute something
+    different."""
     def refuse(what):
-        raise NotImplementedError(f"sfast (H100 build): {what} is not supported by the H100 path (one plain "
-                                  "IP-Adapter with an ImageProjection is)")
+        raise NotImplementedError(f"sfast (H100 build): {what} is not supported by the H100 path (one "
+                                  "IP-Adapter with an ImageProjection or an IPAdapterPlusImageProjection is)")
+    if spec.temporal:
+        refuse("an IP-Adapter on the SVD UNet (UNetSpatioTemporalConditionModel)")
     if getattr(unet, "text_encoder_hid_proj", None) is not None:
         refuse("text_encoder_hid_proj (a text projection next to the IP-Adapter)")
     proj = getattr(unet, "encoder_hid_proj", None)
@@ -308,20 +343,22 @@ def ip_adapter_spec(unet, spec: UNetSpec) -> IPAdapterSpec:
         refuse(f"more than one IP-Adapter at once ({len(layers)} image projections)")
     lay = layers[0]
     kind = type(lay).__name__
-    if kind == "IPAdapterPlusImageProjection":
-        refuse("IPAdapterPlusImageProjection (IP-Adapter Plus, Resampler)")
     if kind in _FACEID_PROJECTIONS:
         refuse(f"{kind} (IP-Adapter FaceID)")
-    if kind != "ImageProjection":
+    if kind == "IPAdapterPlusImageProjection":
+        ip = _resampler_ip_spec(lay, spec, refuse)
+        ctx = ip.ctx_dim
+    elif kind != "ImageProjection":
         refuse(f"image projection {kind}")
-    lin, norm = lay.image_embeds, lay.norm
-    tokens = int(getattr(lay, "num_image_text_embeds", 0) or 0)
-    ctx = int(getattr(lay, "cross_attention_dim", norm.normalized_shape[0]))
-    if ctx != spec.cross_attention_dim or tuple(norm.normalized_shape) != (ctx,) or \
-            tokens <= 0 or lin.out_features != tokens * ctx:
-        refuse(f"ImageProjection geometry (tokens {tokens}, context {ctx}, linear {lin.out_features}, UNet "
-               f"cross_attention_dim {spec.cross_attention_dim})")
-    ip = ip_adapter_geometry(spec, lin.in_features, tokens, norm.eps)
+    else:
+        lin, norm = lay.image_embeds, lay.norm
+        tokens = int(getattr(lay, "num_image_text_embeds", 0) or 0)
+        ctx = int(getattr(lay, "cross_attention_dim", norm.normalized_shape[0]))
+        if ctx != spec.cross_attention_dim or tuple(norm.normalized_shape) != (ctx,) or \
+                tokens <= 0 or lin.out_features != tokens * ctx:
+            refuse(f"ImageProjection geometry (tokens {tokens}, context {ctx}, linear {lin.out_features}, UNet "
+                   f"cross_attention_dim {spec.cross_attention_dim})")
+        ip = ip_adapter_geometry(spec, lin.in_features, tokens, norm.eps)
     dims = dict(spec.cross_attention_layers())
     for prefix in ip.layers:
         proc = getattr(unet.get_submodule(prefix), "processor", None)
@@ -335,6 +372,93 @@ def ip_adapter_spec(unet, spec: UNetSpec) -> IPAdapterSpec:
             if tuple(lin_.weight.shape) != (C, ctx) or getattr(lin_, "bias", None) is not None:
                 refuse(f"{prefix}.processor image K/V projection of shape {tuple(lin_.weight.shape)}")
         ip_scale_of(proc, prefix)
+    return ip
+
+
+_DEFAULT_ATTN_PROCESSORS = ("AttnProcessor2_0", "AttnProcessor")
+
+
+def _resampler_ip_spec(lay, spec: UNetSpec, refuse) -> IPAdapterSpec:
+    """The IPAdapterSpec of an ``IPAdapterPlusImageProjection``, read from the module; everything the plan would
+    compute differently (another head size, a bias diffusers' layers do not have, a non-default attention
+    processor, a tanh GELU, a missing sub-module) is refused by name."""
+    kind = "IPAdapterPlusImageProjection"
+    parts = {n: getattr(lay, n, None) for n in ("latents", "proj_in", "layers", "proj_out", "norm_out")}
+    missing = [n for n, v in parts.items() if v is None]
+    if missing:
+        refuse(f"{kind} without {' / '.join(missing)} (not diffusers' IP-Adapter Plus layout)")
+    lat, proj_in, blocks, proj_out, norm_out = parts.values()
+    if lat.dim() != 3 or lat.shape[0] != 1:
+        refuse(f"{kind}.latents of shape {tuple(lat.shape)} (expected [1, num_queries, hidden_dims])")
+    tokens, dh = int(lat.shape[1]), int(lat.shape[2])
+    ctx = spec.cross_attention_dim
+    if dh % RESAMPLER_HEAD_DIM:
+        refuse(f"{kind} hidden_dims {dh} (not a multiple of {RESAMPLER_HEAD_DIM})")
+    if proj_in.out_features != dh or proj_in.bias is None or proj_out.in_features != dh or \
+            proj_out.out_features != ctx or proj_out.bias is None:
+        refuse(f"{kind} proj_in / proj_out geometry (hidden_dims {dh}, proj_in {tuple(proj_in.weight.shape)}, "
+               f"proj_out {tuple(proj_out.weight.shape)}, UNet cross_attention_dim {ctx})")
+
+    def layer_norm(m, what, c):
+        if m is None or tuple(getattr(m, "normalized_shape", ())) != (c,) or getattr(m, "weight", None) is None \
+                or getattr(m, "bias", None) is None:
+            refuse(f"{kind} {what} (expected an affine LayerNorm over {c})")
+        return float(m.eps)
+
+    def no_bias_linear(m, what, shape):
+        if m is None or tuple(m.weight.shape) != shape:
+            refuse(f"{kind} {what} of shape {None if m is None else tuple(m.weight.shape)} (expected {shape})")
+        if getattr(m, "bias", None) is not None:
+            refuse(f"{kind} {what} with a bias (diffusers' layer has none)")
+
+    norm_eps = layer_norm(norm_out, "norm_out", ctx)
+    blocks = list(blocks)
+    if not blocks:
+        refuse(f"{kind} with no blocks")
+    heads = ff_dim = None
+    block_eps = []
+    for i, blk in enumerate(blocks):
+        b = f"layers.{i}"
+        attn, ff = getattr(blk, "attn", None), getattr(blk, "ff", None)
+        if attn is None or ff is None or not hasattr(attn, "to_q"):
+            refuse(f"{kind} {b} without attn / ff")
+        h = int(getattr(attn, "heads", 0) or 0)
+        inner = attn.to_q.out_features
+        if h <= 0 or inner != h * RESAMPLER_HEAD_DIM:
+            refuse(f"{kind} {b}.attn with dim_head {inner / max(h, 1):g} (heads {h}; dim_head "
+                   f"{RESAMPLER_HEAD_DIM} is)")
+        if heads is not None and h != heads:
+            refuse(f"{kind} with a different head count per block")
+        heads = h
+        proc = getattr(attn, "processor", None)
+        if type(proc).__name__ not in _DEFAULT_ATTN_PROCESSORS:
+            refuse(f"{kind} {b}.attn.processor of type {type(proc).__name__} (diffusers' default "
+                   "AttnProcessor2_0 is)")
+        if abs(float(getattr(attn, "scale", RESAMPLER_HEAD_DIM ** -0.5)) - RESAMPLER_HEAD_DIM ** -0.5) > 1e-12 or \
+                float(getattr(attn, "rescale_output_factor", 1.0)) != 1.0 or \
+                getattr(attn, "residual_connection", False):
+            refuse(f"{kind} {b}.attn with a non-default scale / rescale_output_factor / residual_connection")
+        for n in ("to_q", "to_k", "to_v"):
+            no_bias_linear(getattr(attn, n, None), f"{b}.attn.{n}", (inner, dh))
+        to_out = getattr(attn, "to_out", None)
+        no_bias_linear(to_out[0] if to_out is not None else None, f"{b}.attn.to_out.0", (dh, inner))
+        net = getattr(ff[1], "net", None) if len(ff) == 2 else None
+        if net is None or len(net) != 3 or not hasattr(net[0], "proj"):
+            refuse(f"{kind} {b}.ff (expected Sequential(LayerNorm, FeedForward))")
+        if getattr(net[0], "approximate", "none") != "none" or type(net[0]).__name__ != "GELU":
+            refuse(f"{kind} {b}.ff activation {type(net[0]).__name__}"
+                   f"(approximate={getattr(net[0], 'approximate', None)!r}); the erf GELU is")
+        f = net[0].proj.out_features
+        if ff_dim is not None and f != ff_dim:
+            refuse(f"{kind} with a different FeedForward width per block")
+        ff_dim = f
+        no_bias_linear(net[0].proj, f"{b}.ff.1.net.0.proj", (f, dh))
+        no_bias_linear(net[2], f"{b}.ff.1.net.2", (dh, f))
+        block_eps.append((layer_norm(getattr(blk, "ln0", None), f"{b}.ln0", dh),
+                          layer_norm(getattr(blk, "ln1", None), f"{b}.ln1", dh),
+                          layer_norm(ff[0], f"{b}.ff.0", dh)))
+    ip = ip_adapter_geometry(spec, proj_in.in_features, tokens, norm_eps)
+    ip.resampler = ResamplerSpec(dh, heads, len(blocks), ff_dim, tuple(block_eps))
     return ip
 
 
@@ -553,8 +677,25 @@ def param_shapes(spec: UNetSpec):
     if spec.ip is not None:
         # diffusers' names after load_ip_adapter
         ip, pp = spec.ip, "encoder_hid_proj.image_projection_layers.0"
-        lin(pp + ".image_embeds", ip.tokens * ip.ctx_dim, ip.image_embed_dim)
-        norm(pp + ".norm", ip.ctx_dim)
+        rs = ip.resampler
+        if rs is None:
+            lin(pp + ".image_embeds", ip.tokens * ip.ctx_dim, ip.image_embed_dim)
+            norm(pp + ".norm", ip.ctx_dim)
+        else:
+            out[pp + ".latents"] = (1, ip.tokens, rs.dim)
+            lin(pp + ".proj_in", rs.dim, ip.image_embed_dim)
+            for i in range(rs.depth):
+                b = f"{pp}.layers.{i}"
+                norm(b + ".ln0", rs.dim)
+                norm(b + ".ln1", rs.dim)
+                for n in ("to_q", "to_k", "to_v"):
+                    lin(f"{b}.attn.{n}", rs.inner, rs.dim, False)
+                lin(b + ".attn.to_out.0", rs.dim, rs.inner, False)
+                norm(b + ".ff.0", rs.dim)
+                lin(b + ".ff.1.net.0.proj", rs.ff_dim, rs.dim, False)
+                lin(b + ".ff.1.net.2", rs.dim, rs.ff_dim, False)
+            lin(pp + ".proj_out", ip.ctx_dim, rs.dim)
+            norm(pp + ".norm_out", ip.ctx_dim)
         dims = dict(spec.cross_attention_layers())
         for prefix in ip.layers:
             lin(prefix + ".processor.to_k_ip.0", dims[prefix].dim, ip.ctx_dim, False)
@@ -572,6 +713,8 @@ def random_state_dict(spec: UNetSpec, seed=0, dtype=torch.float16, device="cpu")
         is_norm = ".norm" in name or name.startswith("conv_norm_out")
         if name.endswith("mix_factor"):
             t = torch.randn(shape, generator=g) * 1.5
+        elif name.endswith(".latents"):  # IP-Adapter Plus queries, initialised as diffusers does
+            t = torch.randn(shape, generator=g) / math.sqrt(shape[-1])
         elif is_norm:
             # random affine (not PyTorch's 1 / 0): a benchmark must not hide a dropped beta
             t = torch.randn(shape, generator=g) * 0.3 + (1.0 if name.endswith("weight") else 0.0)

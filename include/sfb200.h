@@ -364,6 +364,16 @@ int sfb_conv_in(const void* x, const void* w, const float* bias, void* y, int32_
 int sfb_conv_out(const void* x, const void* w, const float* bias, void* y, int32_t n, int32_t h,
                  int32_t wd, int32_t cin, int32_t cout, int32_t ldx, int32_t dtype,
                  sfb_stream_t stream);
+/* The tail of SVD's temporal VAE decoder: conv_out then time_conv_out.  The n images of x are
+ * n / frames videos of `frames` consecutive frames (n % frames == 0).
+ *   c[i]    = round16(conv3x3(x[i], w) + bias)           (sfb_conv_out's conv, same x / w / bias layout)
+ *   y[v, f] = bt + sum_k wt[:, k, :] . c[v, f + k - 1]   (k = 0..2; frames -1 and `frames` are zero)
+ * wt: 16-bit [cout, 3, cout] (output channel, frame tap, input channel) -- Conv3d weight
+ * [cout, cout, 3, 1, 1] permuted; bt fp32 (may be NULL).  y NCHW [n, cout<=8, h, w] 16-bit.  c never
+ * reaches memory.  Needs (n / frames) * h * w < 2^31. */
+int sfb_conv_out_temporal(const void* x, const void* w, const float* bias, const void* wt, const float* bt,
+                          void* y, int32_t n, int32_t h, int32_t wd, int32_t cin, int32_t cout, int32_t ldx,
+                          int32_t frames, int32_t dtype, sfb_stream_t stream);
 
 /* nearest-neighbour 2x upsample, NHWC, 16-bit */
 int sfb_upsample2x(const void* x, void* y, int32_t n, int32_t h, int32_t w, int32_t c,

@@ -118,6 +118,7 @@ struct GemmArgs {
     int up_ntiles;  // ... and N tiles per phase in the phase-concatenated weight matrix
     int b_plain;    // B is a plain row-major [N, K] matrix (an activation), not a pre-tiled weight
     int b_half;     // tmap_b has the 80-row box (cta_pair / persistent callers): two loads per B tile
+    int m_tile_base;  // M tile of blockIdx.y == 0: more M tiles than a grid's y extent run as several launches
     // SFB_A_CONV3X3_GN: per-(image, channel) GroupNorm (scale, shift) pairs [img_n][cin][2], SiLU flag
     const float* gn_ab;
     int gn_silu;
@@ -505,7 +506,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int n_tile = blockIdx.x;
-    const int m_tile = blockIdx.y;
+    const int m_tile = args.m_tile_base + blockIdx.y;
     const int split = blockIdx.z;
     const int kb_begin = (int)(((long long)args.nkb_total * split) / args.splits);
     const int kb_end = (int)(((long long)args.nkb_total * (split + 1)) / args.splits);
@@ -1245,14 +1246,22 @@ extern "C" int sfb_gemm(const sfb_gemm_params* p, sfb_stream_t stream_) {
     // cta_pair / persistent describe the caller's tensor maps (tmap_b box = 80 rows); every launch is the
     // one-tile kernel, which loads such a 160-row weight tile as two boxes
     a.b_half = p->cta_pair ? 1 : 0;
-    const dim3 grid(n_tiles, m_tiles, a.splits);
-    int rc;
-    if (gnconv)
-        rc = e.dtype == SFB_BF16 ? launch_gemm_t<3, 1, 1>(ta, tb, a, grid, stream)
-                                 : launch_gemm_t<3, 0, 1>(ta, tb, a, grid, stream);
-    else
-        rc = e.dtype == SFB_BF16 ? launch_gemm_t<kGemmStages, 1>(ta, tb, a, grid, stream)
-                                 : launch_gemm_t<kGemmStages, 0>(ta, tb, a, grid, stream);
+    // gridDim.y is at most 65535: a larger M (e.g. 25 frames of 576 x 1024 = 115,200 tiles) runs as several
+    // launches over consecutive M-tile ranges (an even count each, so CTA pairs stay whole)
+    constexpr int kMaxGridY = 65534;
+    if (m_tiles > kMaxGridY && a.splits != 1)
+        return fail(SFB_ERR_INVALID, "sfb_gemm: %d M tiles with split-K (at most %d)", m_tiles, kMaxGridY);
+    int rc = 0;
+    for (int m0 = 0; m0 < m_tiles && rc == 0; m0 += kMaxGridY) {
+        a.m_tile_base = m0;
+        const dim3 grid(n_tiles, m_tiles - m0 < kMaxGridY ? m_tiles - m0 : kMaxGridY, a.splits);
+        if (gnconv)
+            rc = e.dtype == SFB_BF16 ? launch_gemm_t<3, 1, 1>(ta, tb, a, grid, stream)
+                                     : launch_gemm_t<3, 0, 1>(ta, tb, a, grid, stream);
+        else
+            rc = e.dtype == SFB_BF16 ? launch_gemm_t<kGemmStages, 1>(ta, tb, a, grid, stream)
+                                     : launch_gemm_t<kGemmStages, 0>(ta, tb, a, grid, stream);
+    }
     if (rc) return rc;
     if (p->defer_finish && a.splits > 1) {
         if (e.epi != SFB_EPI_STORE || e.rowstats_out || e.ln_rowstats)

@@ -213,61 +213,140 @@ __global__ void __launch_bounds__(128) im2col_in_kernel(const uint16_t* __restri
 // conv_out: NHWC (pitch ld) -> NCHW (cout <= 8), 3x3 pad 1.  One warp per output pixel; lanes
 // split the 9 * cin/8 (tap, 8-channel vector) items; weights [cout][9][cin] staged in smem.
 // ---------------------------------------------------------------------------------------
+__device__ __forceinline__ void conv_out_stage_weights(const ConvEdgeArgs& a, uint16_t* wsm) {
+    for (int i = threadIdx.x; i < (9 * a.cin * a.cout) / 8; i += blockDim.x)
+        reinterpret_cast<uint4*>(wsm)[i] = reinterpret_cast<const uint4*>(a.w)[i];
+}
+
+// The conv of pixel (yh, xw) of image img without bias, summed over the warp: every lane holds all
+// cout sums (a butterfly reduction gives every lane the same bits).
+__device__ __forceinline__ void conv_out_pixel(const ConvEdgeArgs& a, const uint16_t* wsm, int img, int yh, int xw,
+                                               int lane, float (&acc)[8]) {
+    const int kk = 9 * a.cin;
+    const int nvec = a.cin / 8;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+    for (int it = lane; it < 9 * nvec; it += 32) {
+        const int tap = it / nvec, vec = it - tap * nvec;
+        const int iy = yh + tap / 3 - 1, ix = xw + tap % 3 - 1;
+        if (iy < 0 || iy >= a.h || ix < 0 || ix >= a.wd) continue;
+        const uint4 xv = *reinterpret_cast<const uint4*>(
+            a.x + (((size_t)img * a.h + iy) * a.wd + ix) * a.ld + vec * 8);
+        const uint32_t xw4[4] = {xv.x, xv.y, xv.z, xv.w};
+        float xf[8];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float2 f = unpack2(xw4[i], a.dtype);
+            xf[2 * i] = f.x; xf[2 * i + 1] = f.y;
+        }
+#pragma unroll
+        for (int co = 0; co < 8; ++co) {
+            if (co < a.cout) {
+                const uint4 wv = *reinterpret_cast<const uint4*>(&wsm[co * kk + tap * a.cin + vec * 8]);
+                const uint32_t ww[4] = {wv.x, wv.y, wv.z, wv.w};
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float2 f = unpack2(ww[i], a.dtype);
+                    acc[co] += xf[2 * i] * f.x + xf[2 * i + 1] * f.y;
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int co = 0; co < 8; ++co) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) acc[co] += __shfl_xor_sync(0xffffffffu, acc[co], o);
+    }
+}
+
 __global__ void __launch_bounds__(256) conv_out_kernel(const ConvEdgeArgs a) {
     extern __shared__ uint16_t wsm[];  // [cout][9*cin]
     pdl_launch_dependents();
     pdl_wait();
-    const int kk = 9 * a.cin;
-    for (int i = threadIdx.x; i < (kk * a.cout) / 8; i += blockDim.x)
-        reinterpret_cast<uint4*>(wsm)[i] = reinterpret_cast<const uint4*>(a.w)[i];
+    conv_out_stage_weights(a, wsm);
     __syncthreads();
     const int lane = threadIdx.x & 31;
     const int total = a.n * a.h * a.wd;
-    const int nvec = a.cin / 8;
     for (int p = blockIdx.x * 8 + (threadIdx.x >> 5); p < total; p += gridDim.x * 8) {
         const int xw = p % a.wd;
         const int yh = (p / a.wd) % a.h;
         const int img = p / (a.wd * a.h);
         float acc[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-        for (int it = lane; it < 9 * nvec; it += 32) {
-            const int tap = it / nvec, vec = it - tap * nvec;
-            const int iy = yh + tap / 3 - 1, ix = xw + tap % 3 - 1;
-            if (iy < 0 || iy >= a.h || ix < 0 || ix >= a.wd) continue;
-            const uint4 xv = *reinterpret_cast<const uint4*>(
-                a.x + (((size_t)img * a.h + iy) * a.wd + ix) * a.ld + vec * 8);
-            const uint32_t xw4[4] = {xv.x, xv.y, xv.z, xv.w};
-            float xf[8];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const float2 f = unpack2(xw4[i], a.dtype);
-                xf[2 * i] = f.x; xf[2 * i + 1] = f.y;
-            }
-#pragma unroll
-            for (int co = 0; co < 8; ++co) {
-                if (co < a.cout) {
-                    const uint4 wv = *reinterpret_cast<const uint4*>(&wsm[co * kk + tap * a.cin + vec * 8]);
-                    const uint32_t ww[4] = {wv.x, wv.y, wv.z, wv.w};
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float2 f = unpack2(ww[i], a.dtype);
-                        acc[co] += xf[2 * i] * f.x + xf[2 * i + 1] * f.y;
-                    }
-                }
-            }
-        }
-#pragma unroll
-        for (int co = 0; co < 8; ++co) {
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) acc[co] += __shfl_xor_sync(0xffffffffu, acc[co], o);
-        }
+        conv_out_pixel(a, wsm, img, yh, xw, lane, acc);
         if (lane < a.cout) {
             float v = 0.f;
 #pragma unroll
             for (int co = 0; co < 8; ++co) if (lane == co) v = acc[co];
             v += a.bias ? a.bias[lane] : 0.f;
             store1(a.y, (((size_t)img * a.cout + lane) * a.h + yh) * a.wd + xw, v, a.dtype);
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------
+// conv_out + time_conv_out of SVD's temporal VAE decoder: the 3x3 conv above, rounded to 16 bits,
+// then a Conv3d (3,1,1) with zero padding over the frames of each video.  One warp per output
+// pixel of a video walks its frames with a three-frame window (previous, current, next conv_out
+// values, all lanes holding all channels), so every conv_out value is computed once and never
+// leaves registers.  The images of a.n are videos of `frames` consecutive frames.
+// ---------------------------------------------------------------------------------------
+struct ConvOutTemporalArgs {
+    ConvEdgeArgs e;
+    const uint16_t* wt;  // [cout][3][cout] 16-bit: output channel, frame tap, input channel
+    const float* bt;
+    int frames;
+};
+
+__device__ __forceinline__ void conv_out_frame(const ConvEdgeArgs& a, const uint16_t* wsm, int img, int yh, int xw,
+                                               int lane, float (&c)[8]) {
+    conv_out_pixel(a, wsm, img, yh, xw, lane, c);
+#pragma unroll
+    for (int co = 0; co < 8; ++co) {
+        // rounded to the storage type, as diffusers stores conv_out's output before time_conv_out
+        const float v = c[co] + (co < a.cout && a.bias ? a.bias[co] : 0.f);
+        c[co] = unpack2(pack2(v, 0.f, a.dtype), a.dtype).x;
+    }
+}
+
+__global__ void __launch_bounds__(256) conv_out_temporal_kernel(const ConvOutTemporalArgs t) {
+    extern __shared__ uint16_t wsm[];  // [cout][9*cin]
+    __shared__ float wts[8 * 3 * 8];   // [cout][3][cout]
+    const ConvEdgeArgs& a = t.e;
+    pdl_launch_dependents();
+    pdl_wait();
+    conv_out_stage_weights(a, wsm);
+    for (int i = threadIdx.x; i < a.cout * 3 * a.cout; i += blockDim.x) wts[i] = load1(t.wt, i, a.dtype);
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const int hw = a.h * a.wd;
+    const int total = (a.n / t.frames) * hw;  // (video, pixel) pairs
+    for (int q = blockIdx.x * 8 + (threadIdx.x >> 5); q < total; q += gridDim.x * 8) {
+        const int vid = q / hw, pix = q - vid * hw;
+        const int yh = pix / a.wd, xw = pix - yh * a.wd;
+        const int img0 = vid * t.frames;
+        float prev[8], cur[8], next[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) prev[i] = 0.f;  // frame -1: zero padding
+        conv_out_frame(a, wsm, img0, yh, xw, lane, cur);
+        for (int f = 0; f < t.frames; ++f) {
+            if (f + 1 < t.frames) {
+                conv_out_frame(a, wsm, img0 + f + 1, yh, xw, lane, next);
+            } else {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) next[i] = 0.f;  // frame F: zero padding
+            }
+            if (lane < a.cout) {
+                const float* wr = wts + lane * 3 * a.cout;
+                float v = t.bt ? t.bt[lane] : 0.f;
+#pragma unroll
+                for (int ci = 0; ci < 8; ++ci) {
+                    if (ci < a.cout)
+                        v += wr[ci] * prev[ci] + wr[a.cout + ci] * cur[ci] + wr[2 * a.cout + ci] * next[ci];
+                }
+                store1(a.y, ((size_t)(img0 + f) * a.cout + lane) * hw + pix, v, a.dtype);
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) { prev[i] = cur[i]; cur[i] = next[i]; }
         }
     }
 }
@@ -594,6 +673,46 @@ extern "C" int sfb_conv_out(const void* x, const void* w, const float* bias, voi
                                  static_cast<cudaStream_t>(stream), a);
     if (err != cudaSuccess) return fail(SFB_ERR_CUDA, "conv_out: %s", cudaGetErrorString(err));
     return check_launch("sfb_conv_out");
+}
+
+extern "C" int sfb_conv_out_temporal(const void* x, const void* w, const float* bias, const void* wt,
+                                     const float* bt, void* y, int32_t n, int32_t h, int32_t wd, int32_t cin,
+                                     int32_t cout, int32_t ldx, int32_t frames, int32_t dtype,
+                                     sfb_stream_t stream) {
+    if (!x || !w || !wt || !y || cout <= 0 || cout > 8 || cin <= 0 || cin % 8 || ldx < cin || ldx % 8)
+        return fail(SFB_ERR_INVALID, "conv_out_temporal: unsupported geometry cin=%d cout=%d ldx=%d", cin, cout, ldx);
+    if (n <= 0 || h <= 0 || wd <= 0 || frames <= 0 || n % frames)
+        return fail(SFB_ERR_INVALID, "conv_out_temporal: %d images are not whole videos of %d frames", n, frames);
+    if ((long long)(n / frames) * h * wd > INT32_MAX)
+        return fail(SFB_ERR_INVALID, "conv_out_temporal: more than 2^31 (video, pixel) pairs");
+    const size_t smem = (size_t)9 * cin * cout * 2;
+    constexpr size_t kSmemOptin = 227 * 1024 - 8 * 3 * 8 * sizeof(float);
+    if (smem > kSmemOptin)
+        return fail(SFB_ERR_INVALID, "conv_out_temporal: weights exceed the shared memory limit (227 KB)");
+    if (smem > 48 * 1024 - 8 * 3 * 8 * sizeof(float)) {
+        static PerDeviceOnce attr_once;
+        bool& attr_set = attr_once.flag();
+        if (!attr_set) {
+            cudaError_t err = cudaFuncSetAttribute(conv_out_temporal_kernel,
+                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemOptin);
+            if (err != cudaSuccess)
+                return fail(SFB_ERR_CUDA, "conv_out_temporal: smem attribute: %s", cudaGetErrorString(err));
+            attr_set = true;
+        }
+    }
+    ConvOutTemporalArgs t{};
+    t.e = ConvEdgeArgs{reinterpret_cast<const uint16_t*>(x), reinterpret_cast<const uint16_t*>(w), bias,
+                       reinterpret_cast<uint16_t*>(y), n, h, wd, cin, cout, ldx, dtype};
+    t.wt = reinterpret_cast<const uint16_t*>(wt);
+    t.bt = bt;
+    t.frames = frames;
+    const long long total = (long long)(n / frames) * h * wd;
+    int blocks = (int)((total + 7) / 8);
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    cudaError_t err = launch_pdl(conv_out_temporal_kernel, dim3(blocks), dim3(256), smem,
+                                 static_cast<cudaStream_t>(stream), t);
+    if (err != cudaSuccess) return fail(SFB_ERR_CUDA, "conv_out_temporal: %s", cudaGetErrorString(err));
+    return check_launch("sfb_conv_out_temporal");
 }
 
 extern "C" int sfb_upsample2x(const void* x, void* y, int32_t n, int32_t h, int32_t w, int32_t c,

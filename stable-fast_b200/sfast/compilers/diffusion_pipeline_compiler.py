@@ -152,9 +152,12 @@ def compile_vae(m, config):
     """Replace ``m.decode`` and ``m.encode`` with the H100-native VAE decoder and encoder (reference
     `compile_vae`, :154-190, which wraps the sub-modules in auto-trace hooks).  Both share one packed
     copy of the weights.  `encode` is replaced only where the module has one (img2img and inpainting
-    call it every time).  A VAE without post_quant_conv (SVD's AutoencoderKLTemporalDecoder, whose
-    decode takes num_frames) keeps its own decode.  fp32 calls (force_upcast) and diffusers' tiled
-    encode stay on the module's eager path.  A VAE without a `decode` method is returned unchanged
+    call it every time).  SVD's AutoencoderKLTemporalDecoder (no post_quant_conv) gets the native
+    ``decode(z, num_frames, return_dict=True)``: z holds z.shape[0] / num_frames videos, one launch
+    plan and CUDA graph per (frames, num_frames, latent size, dtype), so the pipeline's chunks of
+    `decode_chunk_size` frames and its shorter last chunk each get their own.  Another VAE without
+    post_quant_conv, or one missing any parameter of that decoder, keeps its own decode.  fp32 calls
+    (force_upcast) and diffusers' tiled encode stay on the module's eager path.  A VAE without a `decode` method is returned unchanged
     with a warning (the reference, too, only hooks what it can trace)."""
     from sfast_b200.runtime import compile_vae_module, require_sm90
     if not hasattr(m, 'decode') or not hasattr(m, 'config'):

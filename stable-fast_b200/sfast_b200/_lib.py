@@ -158,6 +158,8 @@ SYMBOLS = {
     "sfb_im2col_in": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _VP]),
     "sfb_conv_in": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "sfb_conv_out": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
+    "sfb_conv_out_temporal": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32,
+                                        _I32, _VP]),
     "sfb_upsample2x": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "sfb_temporal_attention": (C.c_int, [C.POINTER(TemporalAttnParams), _VP]),
     "sfb_row_broadcast_add": (C.c_int, [C.POINTER(RowOpParams), _VP]),

@@ -493,6 +493,17 @@ def conv_small_op(name, lib, *, x, weight, bias, y: Act, n, h, w, cin, cout, str
               2 * n * ho * wo * cout * 9 * cin, 2 * (n * h * w * cin + n * ho * wo * cout))
 
 
+def conv_out_temporal_op(name, lib, *, x: Act, w, bias, wt, bt, out, frames, dt):
+    """sfb_conv_out_temporal: NCHW out [n, cout, H, W] = time_conv_out(conv_out(x)) over videos of `frames`
+    frames; `w` packed like PackedWeights.conv3x3_plain, `wt` like PackedWeights.time_conv_out."""
+    cout = out.shape[1]
+    return Op(name, lib.sfb_conv_out_temporal,
+              (x.ptr, _ptr(w), _ptr(bias), _ptr(wt), _ptr(bt), _ptr(out), x.n, x.h, x.w, x.c, cout, x.ld, frames,
+               dtype_code(dt)),
+              (x.buf, w, bias, wt, bt, out), 2 * x.rows * cout * (9 * x.c + 3 * cout),
+              2 * (x.rows * x.c + out.numel()))
+
+
 def nhwc_to_nchw_scaled_op(name, lib, *, srcs, dsts, scale, dt):
     """sfb_nhwc_to_nchw_scaled: dsts[i] (NCHW tensors) = scale[i] * srcs[i] (NHWC Acts), one launch."""
     assert 0 < len(srcs) == len(dsts) <= 16

@@ -215,24 +215,35 @@ class PackedWeights:
             return (self._mat(wp), bp, inner)
         return self._get(("geglu", prefix), build)
 
-    def conv3x1_t(self, name, one_minus_alpha_of=None):
+    def _blend_scaled(self, v, mix):
+        """v times the temporal share of an AlphaBlender: `mix` = (mix_factor name, switched).  The blend of
+        the spatial x_s and the temporal x_s + t is  x_s + s * t,  with s = 1 - sigmoid(mix_factor) (the SVD
+        UNet) or, with switch_spatial_to_temporal_mix (SVD's temporal VAE decoder), s = sigmoid(mix_factor)."""
+        if mix is None:
+            return v
+        name, switched = mix
+        alpha = torch.sigmoid(self._raw(name).to(self.device).float())
+        return v * (alpha if switched else 1.0 - alpha)
+
+    def conv3x1_t(self, name, mix=None):
         """Temporal conv weight [cout, cin, 3, 1, 1] -> K-major [cout, (kt, cin)] as a GEMM operand;
-        `one_minus_alpha_of`: name of an AlphaBlender mix_factor -- the weight is pre-scaled by
-        (1 - sigmoid(mix_factor)) so that the blend  alpha * x_s + (1 - alpha) * (x_s + conv(..))
-        = x_s + (1 - alpha) * conv(..)  is a plain residual epilogue."""
+        `mix`: (AlphaBlender mix_factor name, switched) -- the weight is pre-scaled by the blend's temporal
+        share (_blend_scaled), so that the blend is a plain residual epilogue."""
         def build():
             w = self._raw(name).to(self.device).float()
             w = w[:, :, :, 0, 0].permute(0, 2, 1).reshape(w.shape[0], -1)
-            if one_minus_alpha_of is not None:
-                w = w * (1.0 - torch.sigmoid(self._raw(one_minus_alpha_of).to(self.device).float()))
-            return self._mat(w.to(self.dtype).contiguous())
-        return self._get(("c3t", name, one_minus_alpha_of), build)
+            return self._mat(self._blend_scaled(w, mix).to(self.dtype).contiguous())
+        return self._get(("c3t", name, mix), build)
 
-    def f32_scaled(self, name, one_minus_alpha_of):
-        def build():
-            v = self._raw(name).to(device=self.device, dtype=torch.float32)
-            return (v * (1.0 - torch.sigmoid(self._raw(one_minus_alpha_of).to(self.device).float()))).contiguous()
-        return self._get(("f32s", name, one_minus_alpha_of), build)
+    def f32_scaled(self, name, mix):
+        """fp32 vector scaled like conv3x1_t(.., mix) (the temporal conv's bias)."""
+        return self._get(("f32s", name, mix), lambda: self._blend_scaled(
+            self._raw(name).to(device=self.device, dtype=torch.float32), mix).contiguous())
+
+    def time_conv_out(self, name):
+        """Conv3d (3,1,1) weight [cout, cin, 3, 1, 1] as sfb_conv_out_temporal takes it: 16-bit [cout, 3, cin]."""
+        return self._get(("c3tout", name), lambda: self._raw(name).to(self.device)[:, :, :, 0, 0].permute(
+            0, 2, 1).to(self.dtype).contiguous())
 
     def scaled_linear(self, prefix, scale):
         """(Mat of scale * W, fp32 scale * b): a linear layer with a constant folded in."""
@@ -373,8 +384,9 @@ class Plan:
     def _a_matrix(self, x: Act):
         return ops.a_matrix(x.ptr, x.rows, x.c, x.ld)
 
-    def group_norm(self, name, x: Act, prefix, silu, eps):
-        y = self.act("gn_out", x.n, x.h, x.w, x.c)
+    def group_norm(self, name, x: Act, prefix, silu, eps, dst: Act = None):
+        """GroupNorm(+SiLU) of x into `dst` (by default the plan's "gn_out" buffer of x's shape)."""
+        y = dst if dst is not None else self.act("gn_out", x.n, x.h, x.w, x.c)
         slot, sync = self.gn_stats[self._gn_count], self.gn_sync[self._gn_count]
         self._gn_count += 1
         partial, pend = None, self._pending
@@ -597,6 +609,35 @@ class Plan:
 
     def flops(self):
         return sum(op.flops for op in self.all_ops())
+
+
+class VideoPlanMixin:
+    """Emitters of a plan whose batch is `nvid` videos of `F` consecutive frames (both set by the plan) --
+    the SVD UNet and SVD's temporal VAE decoder.  Frames are a batch of images for everything spatial; a
+    temporal operator works on the same token-major [B*F*H*W, C] tensors viewed as [B, F, H*W, C]."""
+
+    def _video_view(self, x: Act):
+        """[B*F, h, w, c] -> [B, F*h, w, c]: GroupNorm statistics over (frames, height, width)."""
+        return Act(x.buf, self.nvid, self.F * x.h, x.w, x.c, ld=x.ld, off=x.off)
+
+    def _frame_view(self, y: Act, like: Act):
+        return Act(y.buf, like.n, like.h, like.w, y.c, ld=y.ld, off=y.off)
+
+    def conv3x1_t(self, name, x: Act, wm, bias, dst: Act, rowbias=None, residual: Act = None):
+        """Conv3d (3,1,1), padding (1,0,0) over the frame axis of x viewed as [B, F, H*W, C]."""
+        S = x.h * x.w
+        box_n, box_h, box_w = ops.conv_tile_box(self.F, S)
+        adesc = ops.a_conv(x.ptr, self.nvid, self.F, S, x.c, x.ld, box_n, box_h, box_w, 1)
+        M = x.rows
+        kw = dict(a=adesc, b=wm, M=M, N=wm.n, K=3 * x.c, dt=self.dt, out=dst.ptr, ldo=dst.ld, bias=bias,
+                  conv=dict(n=self.nvid, h=self.F, w=S, cin=x.c, stride=1, box_n=box_n, box_h=box_h,
+                            box_w=box_w, temporal=True),
+                  keep=(x.buf, dst.buf, wm), splits=1)
+        if rowbias is not None:
+            kw.update(rowbias=rowbias[0], rows_per_img=self.F * S, ld_rowbias=rowbias[1])
+        if residual is not None:
+            kw.update(residual=residual.ptr, ldr=residual.ld)
+        self._emit(self._gemm(name, **kw))
 
 
 class UNetPlan(Plan):

@@ -414,16 +414,27 @@ class CompiledVAE(_CompiledModule):
         self._module = module
         self._eager, self._eager_encode = eager_decode, eager_encode
 
-    def _step(self, kind, plan_cls, input_name, x):
-        """Copy x into the static input `input_name` of the plan of `kind` for x's shape, run it, return a
-        copy of its output."""
+    def _step(self, kind, plan_cls, input_name, x, extra=()):
+        """Copy x into the static input `input_name` of the plan of `kind` for x's shape (and the plan
+        arguments `extra`, which follow the batch), run it, return a copy of its output."""
         B, _, H, W = x.shape
         with self._lock, torch.cuda.device(x.device):
             weights = self._weights_for(x.dtype, x.device)
-            gp = self._graphed((kind, B, H, W, x.dtype, x.device.index), lambda: plan_cls(weights, B, H, W))
+            gp = self._graphed((kind, B, *extra, H, W, x.dtype, x.device.index),
+                               lambda: plan_cls(weights, B, *extra, H, W))
             getattr(gp.plan, input_name).copy_(x, non_blocking=True)
             gp.step()
             return gp.plan.out.clone()
+
+    @staticmethod
+    def _decoder_output(out, return_dict):
+        if not return_dict:
+            return (out,)
+        try:
+            from diffusers.models.autoencoders.vae import DecoderOutput as DO  # type: ignore
+            return DO(sample=out)
+        except Exception:  # noqa: BLE001
+            return DecoderOutput(sample=out)
 
     def decode(self, z, return_dict=True, generator=None):
         from .vae_plan import VAEDecodePlan
@@ -433,14 +444,23 @@ class CompiledVAE(_CompiledModule):
                             "path (the native decoder computes in fp16 / bf16)", z.dtype)
             return self._eager(z, return_dict=return_dict, generator=generator)
         require_sm90(z.device)
-        out = self._step("decode", VAEDecodePlan, "z_in", z)
-        if not return_dict:
-            return (out,)
-        try:
-            from diffusers.models.autoencoders.vae import DecoderOutput as DO  # type: ignore
-            return DO(sample=out)
-        except Exception:  # noqa: BLE001
-            return DecoderOutput(sample=out)
+        return self._decoder_output(self._step("decode", VAEDecodePlan, "z_in", z), return_dict)
+
+    def decode_temporal(self, z, num_frames, return_dict=True):
+        """`AutoencoderKLTemporalDecoder.decode(z, num_frames, return_dict=True)`: z holds z.shape[0] /
+        num_frames videos of num_frames consecutive latent frames."""
+        from .vae_plan import TemporalDecodePlan
+        if z.dtype not in (torch.float16, torch.bfloat16):
+            self._warn_once("decode_dtype", "sfast (H100 build): VAE decode in %s is left on the module's eager "
+                            "path (the native decoder computes in fp16 / bf16)", z.dtype)
+            return self._eager(z, num_frames=num_frames, return_dict=return_dict)
+        num_frames = int(num_frames)
+        if num_frames <= 0 or z.shape[0] % num_frames:
+            raise ValueError(f"sfast (H100 build): temporal VAE decode of {z.shape[0]} latent frames with "
+                             f"num_frames={num_frames}: the frames must be whole videos")
+        require_sm90(z.device)
+        out = self._step("decode_t", TemporalDecodePlan, "z_in", z, extra=(num_frames,))
+        return self._decoder_output(out, return_dict)
 
     def encode(self, x, return_dict=True):
         from .vae_plan import VAEEncodePlan
@@ -464,16 +484,31 @@ class CompiledVAE(_CompiledModule):
         return out_cls(latent_dist=dist)
 
 
+def _has_temporal_decoder(m):
+    """True when m's state dict holds every parameter of SVD's temporal decoder with its shape."""
+    from .vae_plan import vae_spec_from_config, vae_temporal_decoder_param_shapes
+    try:
+        shapes = vae_temporal_decoder_param_shapes(vae_spec_from_config(m.config))
+    except NotImplementedError:
+        return False
+    sd = m.state_dict()
+    return all(k in sd and tuple(sd[k].shape) == tuple(s) for k, s in shapes.items())
+
+
 def compile_vae_module(m, enable_cuda_graph=True):
     """Replace ``m.decode`` and ``m.encode`` of an AutoencoderKL (same module object).  `encode` is
-    replaced only where the module has one and its encoder is supported; `decode` is kept where the VAE's
-    decoder is not the 2-D one (SVD's temporal decoder).  Either entry left alone is logged once."""
+    replaced only where the module has one and its encoder is supported.  A VAE whose decoder is not the
+    2-D one gets the native `decode(z, num_frames, return_dict=True)` of SVD's temporal decoder when its
+    state dict holds every parameter of that decoder; otherwise its decode is kept.  Either entry left
+    alone is logged once."""
     from .vae_plan import vae_encoder_spec_from_config
-    eager_decode = m.decode
+    eager_decode, temporal = m.decode, False
     if temporal_decoder(m.state_dict()):
-        logger.warning("sfast (H100 build): %s has no post_quant_conv (e.g. SVD's temporal decoder): its "
-                       "decode is left on the module's eager path", type(m).__name__)
-        eager_decode = None
+        temporal = _has_temporal_decoder(m)
+        if not temporal:
+            logger.warning("sfast (H100 build): %s has no post_quant_conv and is not SVD's temporal decoder: its "
+                           "decode is left on the module's eager path", type(m).__name__)
+            eager_decode = None
     eager_encode = getattr(m, "encode", None)
     if eager_encode is not None:
         try:
@@ -485,7 +520,11 @@ def compile_vae_module(m, enable_cuda_graph=True):
         return m
     compiled = CompiledVAE(m, eager_decode, eager_encode, enable_cuda_graph)
 
-    if eager_decode is not None:
+    if temporal:
+        def decode(z, num_frames, return_dict=True):
+            return compiled.decode_temporal(z, num_frames, return_dict=return_dict)
+        _install(m, "decode", compiled, decode)
+    elif eager_decode is not None:
         def decode(z, return_dict=True, generator=None):
             return compiled.decode(z, return_dict=return_dict, generator=generator)
         _install(m, "decode", compiled, decode)

@@ -25,10 +25,10 @@ import torch
 
 from . import _lib, ops
 from .ops import Act, EPI_GEGLU, Op, _ptr
-from .plan import UNetPlan, _JoinOp
+from .plan import UNetPlan, VideoPlanMixin, _JoinOp
 
 
-class SVDPlan(UNetPlan):
+class SVDPlan(VideoPlanMixin, UNetPlan):
     def __init__(self, weights, videos, height, width):
         self.nvid = videos
         self.F = weights.spec.num_frames
@@ -99,29 +99,6 @@ class SVDPlan(UNetPlan):
         super().resnet(r, x, xs)
         self.temporal_resnet(r, xs, dst)
 
-    def _video_view(self, x: Act):
-        """[B*F, h, w, c] -> [B, F*h, w, c]: GroupNorm statistics over (frames, height, width)."""
-        return Act(x.buf, self.nvid, self.F * x.h, x.w, x.c, ld=x.ld, off=x.off)
-
-    def _frame_view(self, y: Act, like: Act):
-        return Act(y.buf, like.n, like.h, like.w, y.c, ld=y.ld, off=y.off)
-
-    def conv3x1_t(self, name, x: Act, wm, bias, dst: Act, rowbias=None, residual: Act = None):
-        """Conv3d (3,1,1), padding (1,0,0) over the frame axis of x viewed as [B, F, H*W, C]."""
-        S = x.h * x.w
-        box_n, box_h, box_w = ops.conv_tile_box(self.F, S)
-        adesc = ops.a_conv(x.ptr, self.nvid, self.F, S, x.c, x.ld, box_n, box_h, box_w, 1)
-        M = x.rows
-        kw = dict(a=adesc, b=wm, M=M, N=wm.n, K=3 * x.c, dt=self.dt, out=dst.ptr, ldo=dst.ld, bias=bias,
-                  conv=dict(n=self.nvid, h=self.F, w=S, cin=x.c, stride=1, box_n=box_n, box_h=box_h,
-                            box_w=box_w, temporal=True),
-                  keep=(x.buf, dst.buf, wm), splits=1)
-        if rowbias is not None:
-            kw.update(rowbias=rowbias[0], rows_per_img=self.F * S, ld_rowbias=rowbias[1])
-        if residual is not None:
-            kw.update(residual=residual.ptr, ldr=residual.ld)
-        self._emit(self._gemm(name, **kw))
-
     def temporal_resnet(self, r, xs: Act, dst: Act):
         tp, eps = r.temporal_prefix, (r.eps if r.eps is not None else self.spec.eps)
         a1 = self._frame_view(self.group_norm(tp + ".norm1", self._video_view(xs), tp + ".norm1", True, eps), xs)
@@ -132,8 +109,9 @@ class SVDPlan(UNetPlan):
                        h1, rowbias=(rb_ptr, self.F * self.w.tproj_total))
         a2 = self._frame_view(self.group_norm(tp + ".norm2", self._video_view(h1), tp + ".norm2", True, eps), xs)
         # AlphaBlender folded in: dst = xs + (1 - alpha) * (conv2(a2) + b)
-        self.conv3x1_t(tp + ".conv2", a2, self.w.conv3x1_t(tp + ".conv2.weight", r.mixer),
-                       self.w.f32_scaled(tp + ".conv2.bias", r.mixer), dst, residual=xs)
+        mix = (r.mixer, False)
+        self.conv3x1_t(tp + ".conv2", a2, self.w.conv3x1_t(tp + ".conv2.weight", mix),
+                       self.w.f32_scaled(tp + ".conv2.bias", mix), dst, residual=xs)
 
     # --------------------------------------------------------------------------- transformers
     def _row_op(self, name, fn, *, x: Act, y: Act, vec=None, ldv=0, x2: Act = None, mix=None, stats=None,

@@ -20,7 +20,7 @@ import torch
 
 from . import _lib, ops
 from .ops import Act, Op, _ptr
-from .plan import Plan
+from .plan import Plan, VideoPlanMixin
 from .unet_spec import cfg_get
 
 
@@ -118,6 +118,44 @@ def vae_decoder_param_shapes(spec: VAESpec):
             conv(f"decoder.up_blocks.{i}.upsamplers.0.conv", cout, cout, 3)
     norm("decoder.conv_norm_out", boc[0])
     conv("decoder.conv_out", spec.out_channels, boc[0], 3)
+    return out
+
+
+def decoder_resnets(spec: VAESpec):
+    """(module prefix, cin, cout) of every resnet of the decoder, in schedule order."""
+    c = spec.block_out_channels[-1]
+    out = [(f"decoder.mid_block.resnets.{j}", c, c) for j in (0, 1)]
+    cout = c
+    for i, ch in enumerate(reversed(spec.block_out_channels)):
+        cin, cout = cout, ch
+        out += [(f"decoder.up_blocks.{i}.resnets.{j}", cin if j == 0 else cout, cout)
+                for j in range(spec.layers_per_block + 1)]
+    return out
+
+
+def vae_temporal_decoder_param_shapes(spec: VAESpec):
+    """{diffusers parameter name: shape} of the decoder of `AutoencoderKLTemporalDecoder` (SVD's VAE): the 2-D
+    decoder without post_quant_conv, every resnet a SpatioTemporalResBlock (the 2-D resnet as its
+    `spatial_res_block`, a `temporal_res_block` of two (3,1,1) Conv3d and a learned `time_mixer`), and a
+    (3,1,1) `time_conv_out` after conv_out."""
+    out = {}
+    for k, v in vae_decoder_param_shapes(spec).items():
+        if k.startswith("post_quant_conv."):
+            continue
+        p, sep, rest = k.partition(".resnets.")
+        if sep:
+            j, leaf = rest.split(".", 1)
+            k = f"{p}.resnets.{j}.spatial_res_block.{leaf}"
+        out[k] = v
+    for p, _, c in decoder_resnets(spec):
+        t = p + ".temporal_res_block"
+        for n in ("norm1", "norm2"):
+            out[f"{t}.{n}.weight"] = out[f"{t}.{n}.bias"] = (c,)
+        for n in ("conv1", "conv2"):
+            out[f"{t}.{n}.weight"], out[f"{t}.{n}.bias"] = (c, c, 3, 1, 1), (c,)
+        out[p + ".time_mixer.mix_factor"] = (1,)
+    oc = spec.out_channels
+    out["decoder.time_conv_out.weight"], out["decoder.time_conv_out.bias"] = (oc, oc, 3, 1, 1), (oc,)
     return out
 
 
@@ -263,6 +301,83 @@ class VAEDecodePlan(_VAEPlan):
         y = self.group_norm("decoder.conv_norm_out", x, "decoder.conv_norm_out", True, spec.eps)
         self.conv_out("decoder.conv_out", y, self.w.conv3x3_plain("decoder.conv_out.weight"),
                       self.w.f32("decoder.conv_out.bias"), self.out)
+        self._finish()
+
+
+class TemporalDecodePlan(VideoPlanMixin, _VAEPlan):
+    """Static launch schedule of `AutoencoderKLTemporalDecoder.decode(z, num_frames)` (SVD's VAE) for a fixed
+    (frames, num_frames, latent height, width): NCHW latents [frames, latent_channels, h, w], `frames` / num_frames
+    videos of num_frames consecutive frames -> NCHW frames [frames, out_channels, 8 h, 8 w].
+
+    The 2-D decoder's schedule with every resnet a SpatioTemporalResBlock: the 2-D resnet (vae_resnet) writes
+    x_s, then the temporal resnet -- GroupNorm over (frames, height, width) per video, Conv3d (3,1,1),
+    GroupNorm, Conv3d -- adds its output to x_s IN PLACE (the second conv's residual epilogue), with the
+    learned AlphaBlender folded into that conv: x_s + sigmoid(mix_factor) * conv2(..) (the decoder's blenders
+    switch spatial and temporal, the SVD UNet's do not).  The temporal half reuses the spatial half's
+    GroupNorm output and conv1 buffers; its only new buffers are GroupNorm outputs at the resolutions where
+    the spatial convs apply their GroupNorm themselves (about 6 % over the 2-D decoder's total).  conv_out and
+    time_conv_out run as one kernel (sfb_conv_out_temporal)."""
+
+    def __init__(self, weights, frames, num_frames, height, width):
+        spec = weights.spec
+        if num_frames <= 0 or frames <= 0 or frames % num_frames:
+            raise ValueError(f"sfast (H100 build): {frames} latents are not whole videos of num_frames={num_frames}")
+        if height * width % 64:
+            # the mid-block attention runs P V with the token count as its K
+            raise NotImplementedError(f"sfast (H100 build): temporal VAE decode of a {height}x{width} latent: the "
+                                      "mid-block attention needs a latent of a multiple of 64 pixels")
+        self.nvid, self.F = frames // num_frames, num_frames
+        n_resnets = 2 + len(spec.block_out_channels) * (spec.layers_per_block + 1)
+        # 2 GroupNorms per spatial and 2 per temporal resnet, the attention's and conv_norm_out
+        super().__init__(weights, frames, height, width, n_gn=4 * n_resnets + 2)
+        self.z_in = self._alloc((frames, spec.latent_channels, height, width), self.dt)
+        up = 1 << (len(spec.block_out_channels) - 1)
+        self.out = self._alloc((frames, spec.out_channels, height * up, width * up), self.dt)
+        self._build()
+
+    def st_resnet(self, p, x: Act, dst: Act, cin, cout):
+        """SpatioTemporalResBlock: x_s = spatial_res_block(x) into dst, then in place
+        dst = x_s + sigmoid(mix_factor) * conv2(silu(norm2(conv1(silu(norm1(x_s))))))."""
+        self.vae_resnet(p + ".spatial_res_block", x, dst, cin, cout)
+        t, eps = p + ".temporal_res_block", 1e-5
+        g = self.act("gn_out", dst.n, dst.h, dst.w, cout)
+        self.group_norm(t + ".norm1", self._video_view(dst), t + ".norm1", True, eps, dst=self._video_view(g))
+        h1 = self.act("res_h1", dst.n, dst.h, dst.w, cout)
+        self.conv3x1_t(t + ".conv1", g, self.w.conv3x1_t(t + ".conv1.weight"), self.w.f32(t + ".conv1.bias"), h1)
+        self.group_norm(t + ".norm2", self._video_view(h1), t + ".norm2", True, eps, dst=self._video_view(g))
+        mix = (p + ".time_mixer.mix_factor", True)
+        self.conv3x1_t(t + ".conv2", g, self.w.conv3x1_t(t + ".conv2.weight", mix),
+                       self.w.f32_scaled(t + ".conv2.bias", mix), dst, residual=dst)
+
+    def _build(self):
+        spec, B, H, W = self.spec, self.B, self.H, self.W
+        boc = spec.block_out_channels
+        c = boc[-1]
+        x = self.act("vae_x0", B, H, W, c)
+        self.conv_in("decoder.conv_in", self.z_in, x)
+        m = "decoder.mid_block"
+        a = self.act("vae_x1", B, H, W, c)
+        self.st_resnet(m + ".resnets.0", x, a, c, c)
+        self.vae_attention(m + ".attentions.0", a, x)
+        self.st_resnet(m + ".resnets.1", x, a, c, c)
+        x, cout, h, w = a, c, H, W
+        for i, ch in enumerate(reversed(boc)):
+            cin, cout = cout, ch
+            for j in range(spec.layers_per_block + 1):
+                dst = self.act(f"vae_up{i}_{j % 2}", B, h, w, cout)
+                self.st_resnet(f"decoder.up_blocks.{i}.resnets.{j}", x, dst, cin if j == 0 else cout, cout)
+                x = dst
+            if i != len(boc) - 1:
+                dst = self.act(f"vae_ups{i}", B, 2 * h, 2 * w, cout)
+                self.upconv3x3(f"decoder.up_blocks.{i}.upsamplers.0.conv", x,
+                               f"decoder.up_blocks.{i}.upsamplers.0.conv", dst)
+                x, h, w = dst, 2 * h, 2 * w
+        y = self.group_norm("decoder.conv_norm_out", x, "decoder.conv_norm_out", True, spec.eps)
+        self._emit(ops.conv_out_temporal_op(
+            "decoder.conv_out+time_conv_out", self.lib_or_dry(), x=y,
+            w=self.w.conv3x3_plain("decoder.conv_out.weight"), bias=self.w.f32("decoder.conv_out.bias"),
+            wt=self.w.time_conv_out("decoder.time_conv_out.weight"), bt=self.w.f32("decoder.time_conv_out.bias"),
+            out=self.out, frames=self.F, dt=self.dt))
         self._finish()
 
 

@@ -49,7 +49,7 @@ enum sfb_status {
     SFB_ERR_NO_DRIVER = -3, /* driver entry point unavailable */
 };
 
-enum sfb_dtype { SFB_F16 = 0, SFB_BF16 = 1 };
+enum sfb_dtype { SFB_F16 = 0, SFB_BF16 = 1, SFB_F32 = 2 /* sfb_lora_merge inputs only */ };
 
 int sfb_abi_version(void);
 const char* sfb_last_error(void);
@@ -525,6 +525,36 @@ int sfb_clip_pool(const int64_t* ids, const void* x, void* pooled, int32_t batch
  * row pitch kpad (a multiple of 64 for the GEMM), columns beyond chans * patch^2 zeroed. */
 int sfb_patchify(const void* x, void* a, int32_t batch, int32_t chans, int32_t h, int32_t w, int32_t patch,
                  int32_t kpad, sfb_stream_t stream);
+
+/* ---- LoRA adapters (PEFT LoraLayer, merged into the weights when the adapter state changes; the
+ * reference's recipe is fuse_lora() on the module before compiling) ------------------------------ */
+
+#define SFB_LORA_MAX_ADAPTERS 8
+#define SFB_LORA_MAX_RANK 256
+
+/* One adapter: A [rank, k] (row pitch lda), B [n, rank] (row pitch ldb), each SFB_F16 / SFB_BF16 /
+ * SFB_F32 independently of W; `scale` is PEFT's scaling[adapter] times any call-time factor. */
+typedef struct sfb_lora_adapter {
+    const void* a;
+    const void* b;
+    int32_t rank, lda, ldb, a_dtype, b_dtype;
+    float scale;
+} sfb_lora_adapter;
+
+/* out[n, k] = round(W[n, k] + sum_i scale_i * sum_j B_i[n, j] A_i[j, k]), fp32 arithmetic and ONE rounding
+ * to out_dtype (SFB_F16 / SFB_BF16) at the end.  W [n, k] (row pitch ldw) is SFB_F16 / SFB_BF16 / SFB_F32;
+ * out (row pitch ldo) is caller-owned and must not alias W, A or B.  A conv weight [cout, cin, kh, kw] is
+ * W [cout, cin*kh*kw] with A the lora_A conv weight [rank, cin*kh*kw] (OIHW order) and B the 1x1 lora_B
+ * weight [cout, rank].  1 <= count <= SFB_LORA_MAX_ADAPTERS, 1 <= rank <= SFB_LORA_MAX_RANK. */
+typedef struct sfb_lora_merge_params {
+    const void* w;
+    void* out;
+    int32_t n, k, ldw, ldo, w_dtype, out_dtype;
+    int32_t count;
+    sfb_lora_adapter adapters[SFB_LORA_MAX_ADAPTERS];
+} sfb_lora_merge_params;
+
+int sfb_lora_merge(const sfb_lora_merge_params* p, sfb_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -14,9 +14,10 @@ Field mapping (all 11 reference fields are accepted):
                          -> accepted; they select nothing: the native path always runs NHWC with
                             every fusion on (fp32 accumulation, erf-GELU)
   preserve_parameters    -> True (default): in-place parameter updates (LoRA switch, reference
-                            README.md:228-265) are picked up by the next call -- the packed copies
-                            are refreshed in place when the parameters' version counters move;
-                            False: weights are frozen at first call (``rebind()`` refreshes)
+                            README.md:228-265) and PEFT LoRA adapter changes are picked up by the next
+                            call -- the packed copies are refreshed in place;
+                            False: weights and adapter state are frozen at first call (``rebind()``
+                            refreshes)
   trace_scheduler        -> accepted, no-op (scheduler is outside the hot path)
 """
 import logging
@@ -53,7 +54,9 @@ def compile(m, config):
     ControlNet (``pipe.controlnet``: a ControlNetModel, or each net of a MultiControlNetModel), the VAE, the
     text encoders and the image encoder run on the native path; a ControlNet class or config the native
     path does not cover stays eager with a warning.  A loaded IP-Adapter (one plain ``ImageProjection`` or one
-    IP-Adapter Plus ``IPAdapterPlusImageProjection``) runs inside the UNet's step, see `compile_unet`."""
+    IP-Adapter Plus ``IPAdapterPlusImageProjection``) runs inside the UNet's step, see `compile_unet`.  PEFT LoRA
+    adapters on the UNet and the text encoders are merged into their packed weights (see `compile_unet`); adapters
+    on the ControlNet, the VAE or the vision tower raise ``NotImplementedError`` at their first call."""
     m.unet = compile_unet(m.unet, config)
     if getattr(m, 'controlnet', None) is not None:
         m.controlnet = compile_controlnet(m.controlnet, config)
@@ -139,7 +142,13 @@ def compile_unet(m, config):
     compiled with it: a plain adapter's image projection, or IP-Adapter Plus's Resampler (its perceiver blocks
     over the image features of ``added_cond_kwargs["image_embeds"]``, ``[B, n_img, S_img, D_img]``), runs on
     the step's side stream inside the same CUDA graph, and every cross-attention adds the image-token term.
-    FaceID projections, several adapters and ``ip_adapter_masks`` raise ``NotImplementedError`` by name."""
+    FaceID projections, several adapters and ``ip_adapter_masks`` raise ``NotImplementedError`` by name.
+
+    PEFT LoRA adapters (diffusers' ``load_lora_weights``), loaded before or after this call, fused or not, are
+    merged into the packed weights whenever the adapter state changes (``set_adapters``, ``fuse_lora``,
+    ``disable_lora``, ``delete_adapters``, ...); ``cross_attention_kwargs={"scale": s}`` scales the active
+    adapters for that call.  The step's launch list and CUDA graph are those of the adapter-free UNet.  DoRA,
+    ``lora_bias`` and non-LoRA PEFT adapters raise ``NotImplementedError`` naming the layer."""
     from sfast_b200.runtime import compile_unet_module, require_sm90
     device = m.device if hasattr(m, 'device') else torch.device(
         'cuda' if torch.cuda.is_available() else 'cpu')

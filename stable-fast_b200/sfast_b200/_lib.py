@@ -11,7 +11,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SFB_LIB_PATH") or os.path.join(_HERE, "libsfb200.so")
 
 ABI_VERSION = 4  # SFB_ABI_VERSION of include/sfb200.h
-SFB_F16, SFB_BF16 = 0, 1
+SFB_F16, SFB_BF16, SFB_F32 = 0, 1, 2
+LORA_MAX_ADAPTERS, LORA_MAX_RANK = 8, 256
 A_MATRIX, A_CONV3X3, A_UPCONV2X, A_CONV3X1, A_CONV3X3_GN, A_DOWNCONV3X3 = 0, 1, 2, 3, 4, 5
 ROW_IDX_DIV_MOD, ROW_IDX_TEMPORAL_CTX = 0, 1
 EPI_STORE, EPI_GEGLU, EPI_QKV, EPI_STORE_F32 = 0, 1, 2, 3
@@ -133,6 +134,17 @@ class NhwcToNchwParams(C.Structure):
     _fields_ = [("count", C.c_int32), ("dtype", C.c_int32), ("scale", C.c_void_p), ("items", NchwScaledItem * 16)]
 
 
+class LoraAdapter(C.Structure):
+    _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("rank", C.c_int32), ("lda", C.c_int32), ("ldb", C.c_int32),
+                ("a_dtype", C.c_int32), ("b_dtype", C.c_int32), ("scale", C.c_float)]
+
+
+class LoraMergeParams(C.Structure):
+    _fields_ = [("w", C.c_void_p), ("out", C.c_void_p), ("n", C.c_int32), ("k", C.c_int32), ("ldw", C.c_int32),
+                ("ldo", C.c_int32), ("w_dtype", C.c_int32), ("out_dtype", C.c_int32), ("count", C.c_int32),
+                ("adapters", LoraAdapter * LORA_MAX_ADAPTERS)]
+
+
 # every symbol include/sfb200.h declares: (name, restype, argtypes)
 _I32, _U32, _U64, _VP, _F = C.c_int32, C.c_uint32, C.c_uint64, C.c_void_p, C.c_float
 SYMBOLS = {
@@ -175,6 +187,7 @@ SYMBOLS = {
     "sfb_patchify": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "sfb_conv3x3_small": (C.c_int, [C.POINTER(ConvSmallParams), _VP]),
     "sfb_nhwc_to_nchw_scaled": (C.c_int, [C.POINTER(NhwcToNchwParams), _VP]),
+    "sfb_lora_merge": (C.c_int, [C.POINTER(LoraMergeParams), _VP]),
 }
 
 _lib = None

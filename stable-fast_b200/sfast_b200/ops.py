@@ -643,6 +643,58 @@ def pack_geglu(w, b, dt, extra=None):
     return wp, bp, inner
 
 
+_ANY_DTYPE = {torch.float16: _lib.SFB_F16, torch.bfloat16: _lib.SFB_BF16, torch.float32: _lib.SFB_F32}
+
+
+def lora_merge_params(w, adapters, out):
+    """Validated sfb_lora_merge argument block for out = round(w + sum_i s_i * B_i A_i).  w: [n, k] (fp16 / bf16 /
+    fp32, unit column stride); adapters: 1..8 tuples (A [r, k], B [n, r], s) with 1 <= r <= 256, A and B each fp16
+    / bf16 / fp32; out: fp16 / bf16 [n, k], unit column stride, sharing no memory with the inputs.  Row pitches
+    are taken from the tensors' strides.  Raises ValueError naming what is wrong."""
+    if w.dim() != 2 or out.dim() != 2 or tuple(out.shape) != tuple(w.shape):
+        raise ValueError(f"lora_merge: W {tuple(w.shape)} and out {tuple(out.shape)} must be the same 2-D shape")
+    n, k = w.shape
+    if w.dtype not in _ANY_DTYPE or out.dtype not in (torch.float16, torch.bfloat16):
+        raise ValueError(f"lora_merge: W {w.dtype} must be fp16 / bf16 / fp32 and out {out.dtype} fp16 / bf16")
+    if not 1 <= len(adapters) <= _lib.LORA_MAX_ADAPTERS:
+        raise ValueError(f"lora_merge: {len(adapters)} adapters; 1..{_lib.LORA_MAX_ADAPTERS} per launch")
+    mats = [w, out]
+    p = _lib.LoraMergeParams()
+    for i, (a, b, s) in enumerate(adapters):
+        if a.dim() != 2 or b.dim() != 2:
+            raise ValueError(f"lora_merge: adapter {i}: A and B must be 2-D")
+        r = a.shape[0]
+        if tuple(a.shape) != (r, k) or tuple(b.shape) != (n, r):
+            raise ValueError(f"lora_merge: adapter {i}: A {tuple(a.shape)} / B {tuple(b.shape)} do not fit W "
+                             f"{(n, k)}: expected A [r, {k}] and B [{n}, r]")
+        if not 1 <= r <= _lib.LORA_MAX_RANK:
+            raise ValueError(f"lora_merge: adapter {i}: rank {r}; 1..{_lib.LORA_MAX_RANK}")
+        if a.dtype not in _ANY_DTYPE or b.dtype not in _ANY_DTYPE:
+            raise ValueError(f"lora_merge: adapter {i}: A {a.dtype} / B {b.dtype} must be fp16 / bf16 / fp32")
+        ad = p.adapters[i]
+        ad.a, ad.b, ad.rank, ad.lda, ad.ldb = _ptr(a), _ptr(b), r, a.stride(0), b.stride(0)
+        ad.a_dtype, ad.b_dtype, ad.scale = _ANY_DTYPE[a.dtype], _ANY_DTYPE[b.dtype], float(s)
+        mats += [a, b]
+    for t in mats:
+        if t.stride(1) != 1 and t.shape[1] > 1:
+            raise ValueError("lora_merge: every operand needs unit column stride (rows may be pitched)")
+        if t.device != w.device:
+            raise ValueError(f"lora_merge: operands on {t.device} and {w.device}")
+    if any(out.untyped_storage().data_ptr() == t.untyped_storage().data_ptr() for t in mats[:1] + mats[2:]):
+        raise ValueError("lora_merge: out shares memory with W, A or B")
+    p.w, p.out, p.n, p.k, p.ldw, p.ldo = _ptr(w), _ptr(out), n, k, w.stride(0), out.stride(0)
+    p.w_dtype, p.out_dtype, p.count = _ANY_DTYPE[w.dtype], dtype_code(out.dtype), len(adapters)
+    return p
+
+
+def lora_merge(w, adapters, out_dtype):
+    """sfb_lora_merge on the current stream into a new [n, k] tensor of out_dtype (see lora_merge_params)."""
+    out = torch.empty(w.shape, dtype=out_dtype, device=w.device)
+    p = lora_merge_params(w, adapters, out)
+    check(_lib.lib().sfb_lora_merge(C.byref(p), torch.cuda.current_stream(w.device).cuda_stream), "sfb_lora_merge")
+    return out
+
+
 def fold_layer_norm(w, b, gamma, beta, dt):
     """Fold LayerNorm(gamma, beta) into the following linear layer y = LN(x) W^T + b:
     returns (W' = W * gamma in the 16-bit type, bias' = beta W^T + b, colsum = sum_k W'[n, k]

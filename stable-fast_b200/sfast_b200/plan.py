@@ -48,6 +48,8 @@ class PackedWeights:
         self.sd = state_dict
         self._cache = {}
         self._builders = {}
+        self._deps = {}        # builder key -> the state-dict names its build read
+        self._reading = None
         # all per-resnet time projections as ONE [sum(cout), temb_dim] matrix
         self.tproj_off = {}
         off = 0
@@ -65,18 +67,36 @@ class PackedWeights:
                 torch.cat(bs, 0).to(device=self.device, dtype=torch.float32).contiguous())
 
     def _raw(self, name):
+        """The state-dict tensor `name`, read once per build (an adapted weight is merged on each read)."""
+        if self._reading is not None and name in self._reading:
+            return self._reading[name]
         if name not in self.sd:
             raise KeyError(f"UNet state dict has no parameter {name!r}")
-        return self.sd[name].detach()
+        t = self.sd[name].detach()
+        if self._reading is not None:
+            self._reading[name] = t
+        return t
+
+    def _build(self, key, builder):
+        outer, self._reading = self._reading, {}
+        try:
+            out = builder()
+            self._deps[key] = frozenset(self._reading)
+        finally:
+            inner, self._reading = self._reading, outer
+            if outer is not None:
+                outer.update(inner)
+        return out
 
     def _get(self, key, builder):
         if key not in self._cache:
-            self._cache[key] = builder()
+            self._cache[key] = self._build(key, builder)
             self._builders[key] = builder
         return self._cache[key]
 
-    def refresh(self, state_dict):
-        """Re-pack from `state_dict` into the existing device tensors (addresses unchanged)."""
+    def refresh(self, state_dict, names=None):
+        """Re-pack from `state_dict` into the existing device tensors (addresses unchanged).  `names`: re-run only
+        the builders that read one of these state-dict names (an adapter change); returns how many ran."""
         self.sd = state_dict
 
         def copy_into(old, new):
@@ -90,12 +110,16 @@ class PackedWeights:
             elif old != new:
                 raise RuntimeError("UNet architecture changed under a compiled module")
 
+        ran = 0
         for key, builder in self._builders.items():
-            copy_into(self._cache[key], builder())
+            if names is None or not self._deps[key].isdisjoint(names):
+                copy_into(self._cache[key], self._build(key, builder))
+                ran += 1
+        return ran
 
     def f32(self, name):
         return self._get(("f32", name), lambda: self._raw(name).to(
-            device=self.device, dtype=torch.float32).contiguous())
+            device=self.device, dtype=torch.float32, memory_format=torch.contiguous_format, copy=True))
 
     def _mat(self, w):
         return ops.Mat(w, self.dry)
@@ -281,8 +305,9 @@ class PackedWeights:
             self._raw(name).to(device=self.device, dtype=torch.float32), (0, n - self._raw(name).shape[0])))
 
     def small(self, name):
+        # (copy=True: a packed tensor never aliases the parameter; refresh() writes into it)
         return self._get(("small", name), lambda: self._raw(name).to(
-            device=self.device, dtype=self.dtype).contiguous())
+            device=self.device, dtype=self.dtype, memory_format=torch.contiguous_format, copy=True))
 
 
 class Plan:

@@ -9,11 +9,13 @@ graphs.py:229-231).
 """
 import functools
 import logging
+import math
 import threading
 import time
 
 import torch
 
+from . import lora
 from .plan import PackedWeights, UNetPlan
 from .svd_plan import SVDPlan
 from .unet_spec import cfg_get, ip_adapter_spec, ip_scale_of, spec_from_config
@@ -83,11 +85,14 @@ class _CompiledModule:
 
     Reference contract (preserve_parameters=True): an in-place parameter update is seen by the next call.
     The packed weights are copies, so the parameters' version counters are compared on every call and the
-    copies refreshed in place when they moved."""
+    copies refreshed in place when they moved.
+
+    `lora_module`: the torch module whose PEFT LoRA layers are merged into the packed weights
+    (lora.LoraTracker); without it, a module carrying adapters is refused by name when its weights are packed."""
 
     _what = "module"  # for log messages
 
-    def __init__(self, spec, state_dict_fn, enable_cuda_graph=True, preserve_parameters=True):
+    def __init__(self, spec, state_dict_fn, enable_cuda_graph=True, preserve_parameters=True, lora_module=None):
         self.spec = spec
         self._state_dict_fn = state_dict_fn
         self.enable_cuda_graph = enable_cuda_graph
@@ -98,6 +103,13 @@ class _CompiledModule:
         self._cached = {}
         self._lock = threading.Lock()
         self._warned = set()
+        self._lora = lora.LoraTracker(lora_module, self._what) if isinstance(lora_module, torch.nn.Module) else None
+        self._lora_scale = 1.0      # call-time LoRA scale merged into the packed weights
+        self._lora_states = None    # adapter state of the next (re-)pack
+        self._lora_frozen = False   # preserve_parameters=False: adapter state frozen until rebind()
+        self._repack_all = False    # a re-pack failed part-way: the next one re-runs every packer
+        # a module whose adapters are not merged: PEFT's peft_config appearing on it is refused at the next call
+        self._unmerged_module = None if self._lora is not None else getattr(state_dict_fn, "__self__", None)
 
     def _warn_once(self, what, msg, *args):
         if what not in self._warned:
@@ -108,36 +120,89 @@ class _CompiledModule:
         self._param_refs = [t for t in sd.values() if torch.is_tensor(t)]
         self._param_versions = [t._version for t in self._param_refs]
 
-    def _weights_for(self, dtype, device):
+    def _weights_for(self, dtype, device, lora_scale=1.0):
         """The packed weights for (dtype, device): packed on first use and re-packed when either changes (the
-        plans of the old copy are dropped); refreshed in place when the parameters' version counters moved.
-        The caller holds the lock and `device` is current."""
-        w = self._weights
+        plans of the old copy are dropped); refreshed in place when the parameters' version counters moved, and
+        the layers whose LoRA adapter state changed (at `lora_scale`, the call's LoRA scale) re-merged and
+        re-packed.  The caller holds the lock and `device` is current."""
+        w, lo = self._weights, self._lora
         if w is None or w.dtype != dtype or w.device != device:
             logger.info("Packing %s weights for the H100 path (%s, %s)", self._what, dtype, device)
+            self._poll_lora(lora_scale)
             sd = self._state_dict_fn()
-            self._weights = PackedWeights(self.spec, sd, dtype, device)
+            self._weights = PackedWeights(self.spec, self._packed_state_dict(sd, dtype, device), dtype, device)
+            self._applied()
             self._track(sd)
             self._cached.clear()
-        elif self.preserve_parameters and [t._version for t in self._param_refs] != self._param_versions:
-            logger.info("%s parameters changed in place: refreshing the packed weights", self._what)
-            self._refresh_locked()
+        elif self.preserve_parameters or (lo is not None and not self._lora_frozen):
+            if lo is None and getattr(self._unmerged_module, "peft_config", None) is not None:
+                lora.refuse_adapters(self._state_dict_fn(), self._what)
+            changed = self._poll_lora(lora_scale)
+            if self._repack_all or (self.preserve_parameters
+                                    and [t._version for t in self._param_refs] != self._param_versions):
+                logger.info("%s parameters changed in place: refreshing the packed weights", self._what)
+                self._refresh_locked()
+            elif changed:
+                logger.info("%s LoRA adapter state changed: re-merging %d layers", self._what, len(changed))
+                self._refresh_locked({p + ".weight" for p in changed})
+        elif lo is not None and not math.isclose(lora_scale, self._lora_scale, rel_tol=lora.SCALE_RTOL):
+            raise NotImplementedError(
+                f"sfast (H100 build): LoRA scale {lora_scale} differs from the scale {self._lora_scale} frozen into the "
+                f"packed {self._what} weights (preserve_parameters=False); call rebind() to re-merge")
+        if lora_scale != 1.0 and (lo is None or not lo.layers):
+            raise NotImplementedError("sfast (H100 build): cross_attention_kwargs (LoRA scale) "
+                                      "is not supported; fuse the LoRA weights into the parameters")
+        self._lora_frozen = not self.preserve_parameters
         return self._weights
 
-    def _refresh_locked(self):
+    def _poll_lora(self, lora_scale):
+        """Prefixes of the LoRA layers whose adapter state changed; keeps their state for the next re-pack."""
+        if self._lora is None:
+            return set()
+        changed, self._lora_states = self._lora.poll(lora_scale)
+        self._lora_scale = lora_scale
+        return changed
+
+    def _packed_state_dict(self, sd, dtype, device):
+        """What PackedWeights reads: the state dict itself, or, with LoRA layers, their merged weights under
+        diffusers' names (the polled adapter state)."""
+        if self._lora is None:
+            lora.refuse_adapters(sd, self._what)
+            return sd
+        return self._lora.view(sd, self._lora_states, dtype, device, dry=False)
+
+    def _applied(self):
+        """The polled adapter state is now in the packed weights."""
+        if self._lora is not None:
+            self._lora.applied = self._lora_states
+
+    def _refresh_locked(self, names=None):
         sd = self._state_dict_fn()
         torch.cuda.current_stream().synchronize()  # no replay may be reading the old values
-        self._weights.refresh(sd)
+        w = self._weights
+        sd_packed = self._packed_state_dict(sd, w.dtype, w.device)
+        try:
+            w.refresh(sd_packed) if names is None else w.refresh(sd_packed, names)
+        except BaseException:
+            # some packers may hold the new state and others the old one: nothing is marked applied, and the
+            # next call re-packs everything (or raises again)
+            self._repack_all = True
+            raise
+        self._repack_all = False
+        self._applied()
         self._track(sd)
 
     def rebind(self):
         """Re-pack the weights now (same device storage: plans and CUDA graphs stay valid).
         Only needed with preserve_parameters=False or after replacing parameter objects in a way
-        the version counters cannot see."""
+        the version counters cannot see.  With preserve_parameters=False it also releases the frozen LoRA
+        adapter state: the next call merges the adapters and LoRA scale current at that call."""
         with self._lock:
             if self._weights is not None:
                 with torch.cuda.device(self._weights.device):
+                    self._poll_lora(self._lora_scale)
                     self._refresh_locked()
+                    self._lora_frozen = False
 
     def _graphed(self, key, make_plan):
         """The plan + graph cached under `key`, built by make_plan() on first use (caller holds the lock)."""
@@ -167,7 +232,10 @@ class CompiledUNet(_CompiledModule):
         """`module`: the UNet itself.  It is where a loaded IP-Adapter lives (``encoder_hid_proj`` and the
         cross-attention processors, whose ``scale`` is read on every call); without it no adapter can be
         compiled."""
-        super().__init__(spec_from_config(config), state_dict_fn, enable_cuda_graph, preserve_parameters)
+        spec = spec_from_config(config)
+        # PEFT LoRA layers are merged into the 2-D UNet's weights; the SVD UNet refuses them by name
+        super().__init__(spec, state_dict_fn, enable_cuda_graph, preserve_parameters,
+                         lora_module=None if spec.temporal else module)
         self.first_call_s = None  # wall time of the first call (packing + plan + capture)
         self._module = module
         self._ip_proj = getattr(module, "encoder_hid_proj", None)
@@ -277,9 +345,10 @@ class CompiledUNet(_CompiledModule):
                 raise NotImplementedError(f"sfast (H100 build): UNet argument `{k}` is not supported")
         B, _, H, W = sample.shape
         ip_len, ip_seq, image_embeds, ip_scales = self._ip_inputs(added_cond_kwargs, cross_attention_kwargs, B)
+        lora_scale = 1.0
         if cross_attention_kwargs:
-            scale = cross_attention_kwargs.get("scale", 1.0)
-            if set(cross_attention_kwargs) - {"scale"} or scale != 1.0:
+            lora_scale = float(cross_attention_kwargs.get("scale", 1.0))
+            if set(cross_attention_kwargs) - {"scale"} or (lora_scale != 1.0 and (self._lora is None or self._lora.quiet())):
                 raise NotImplementedError("sfast (H100 build): cross_attention_kwargs (LoRA scale) "
                                           "is not supported; fuse the LoRA weights into the parameters")
         require_sm90(sample.device)
@@ -294,7 +363,7 @@ class CompiledUNet(_CompiledModule):
         # everything below (allocation, TMA maps, launches, capture) targets sample's device
         with self._lock, torch.cuda.device(sample.device):
             t_first = time.perf_counter() if self.first_call_s is None else None
-            weights = self._weights_for(dtype, sample.device)
+            weights = self._weights_for(dtype, sample.device, lora_scale)
             gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index, controlnet, ip_len, ip_seq),
                                lambda: UNetPlan(weights, B, H, W, ctx_len, controlnet=controlnet, ip_len=ip_len,
                                                 ip_seq=ip_seq))
@@ -542,8 +611,9 @@ class _CompiledClip(_CompiledModule):
 
     _weight0 = _input = _embeds = _proj_output = None
 
-    def __init__(self, spec, config, state_dict_fn, eager_forward, with_projection, enable_cuda_graph=True):
-        super().__init__(spec, state_dict_fn, enable_cuda_graph)
+    def __init__(self, spec, config, state_dict_fn, eager_forward, with_projection, enable_cuda_graph=True,
+                 lora_module=None):
+        super().__init__(spec, state_dict_fn, enable_cuda_graph, lora_module=lora_module)
         self._eager = eager_forward
         self.with_projection = with_projection
         rd = cfg_get(config, "return_dict", None)
@@ -555,7 +625,7 @@ class _CompiledClip(_CompiledModule):
 
     def _run(self, x, key, make_plan, call, output_hidden_states, return_dict):
         if self._weights is None:
-            dtype = self._state_dict_fn()[self._weight0].dtype
+            dtype = lora.plain_state_dict(self._state_dict_fn())[self._weight0].dtype
             if dtype not in (torch.float16, torch.bfloat16):
                 return self._route_eager(f"{dtype} weights: the native encoder computes in fp16 / bf16", call)
         else:
@@ -594,10 +664,12 @@ class CompiledTextEncoder(_CompiledClip):
     _weight0, _input = "text_model.embeddings.token_embedding.weight", "ids_in"
     _embeds, _proj_output = "text_embeds", "CLIPTextModelOutput"
 
-    def __init__(self, config, state_dict_fn, eager_forward, with_projection, enable_cuda_graph=True):
+    def __init__(self, config, state_dict_fn, eager_forward, with_projection, enable_cuda_graph=True, module=None):
+        """`module`: the encoder itself, whose PEFT LoRA layers are merged into the packed weights (their scale
+        is read on every call, so diffusers' scale_lora_layers around the call is honoured)."""
         from .clip_plan import clip_text_spec_from_config
         super().__init__(clip_text_spec_from_config(config, with_projection), config, state_dict_fn, eager_forward,
-                         with_projection, enable_cuda_graph)
+                         with_projection, enable_cuda_graph, lora_module=module)
 
     def __call__(self, input_ids=None, attention_mask=None, position_ids=None, output_attentions=None,
                  output_hidden_states=None, return_dict=None, **kwargs):
@@ -690,7 +762,7 @@ def _clip_output(kind, **fields):
 def compile_text_encoder_module(m, enable_cuda_graph=True):
     """Replace ``m.forward`` of a CLIPTextModel / CLIPTextModelWithProjection (same module object)."""
     compiled = CompiledTextEncoder(m.config, m.state_dict, m.forward, hasattr(m, "text_projection"),
-                                   enable_cuda_graph)
+                                   enable_cuda_graph, module=m)
 
     def forward(*args, **kwargs):
         if args:

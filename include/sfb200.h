@@ -467,6 +467,59 @@ typedef struct sfb_conv_small_params {
 
 int sfb_conv3x3_small(const sfb_conv_small_params* p, sfb_stream_t stream);
 
+/* sfb_conv3x3_small with an element-wise transform of the input and a ReLU option (the edge convolutions of
+ * diffusers' AutoencoderTiny).  in_xform is applied to in-image input values only, so the zero padding stays
+ * zero (which is why it cannot be folded into the weights); it needs the NCHW input (base.x_nchw = 1).
+ * relu: 1 applies ReLU after the bias (base.silu must then be 0). */
+enum sfb_conv_xform {
+    SFB_XFORM_NONE = 0,
+    SFB_XFORM_TANH3 = 1, /* tanh(x / 3) * 3   (DecoderTiny's latent clamp) */
+    SFB_XFORM_UNIT = 2,  /* (x + 1) / 2       (EncoderTiny's [-1, 1] -> [0, 1]) */
+};
+
+typedef struct sfb_conv_small_ex_params {
+    sfb_conv_small_params base;
+    int32_t in_xform; /* enum sfb_conv_xform */
+    int32_t relu;
+} sfb_conv_small_ex_params;
+
+int sfb_conv3x3_small_ex(const sfb_conv_small_ex_params* p, sfb_stream_t stream);
+
+/* ---- AutoencoderTiny (TAESD / TAESDXL; the reference compiles it through the same auto-trace hooks as
+ * any VAE, compilers/diffusion_pipeline_compiler.py:154-190) ------------------------------------------ */
+
+enum sfb_c64_mode {
+    SFB_C64_SAME = 0,    /* stride 1, zero padding 1: output h x w */
+    SFB_C64_STRIDE2 = 1, /* stride 2, zero padding 1 on EVERY side (nn.Conv2d(stride=2, padding=1)): output
+                          * ceil(h / 2) x ceil(w / 2); output row i reads input rows 2i - 1 .. 2i + 1 */
+    SFB_C64_UP2X = 2,    /* nearest-2x upsample of x, then stride 1, padding 1: output 2h x 2w, computed from the
+                          * h x w input (the upsampled tensor never exists) */
+};
+
+/* 3x3 convolution with cin = cout = 64, fp32 accumulation on tensor cores, 16-bit storage:
+ *   y = relu?(conv(x) + bias (+ residual))
+ *   x:        NHWC [n, h, w, 64], channel pitch ldx (input dims; `mode` gives the output dims ho x wo);
+ *   weight:   16-bit [64, 3, 3, 64] (cout, kh, kw, cin), contiguous -- [64, 576] K-major;
+ *   bias:     fp32 [64] or NULL;
+ *   residual: NHWC [n, ho, wo, 64] 16-bit, channel pitch ldr, or NULL; may be y itself (in place);
+ *   y:        NHWC [n, ho, wo, 64], channel pitch ldy;
+ *   relu:     1 applies ReLU last (after the residual add).
+ * Pitches are multiples of 8 and at least 64; every pointer is 16-byte aligned; x must not overlap y. */
+typedef struct sfb_conv_c64_params {
+    const void* x;
+    const void* weight;
+    const float* bias;
+    const void* residual;
+    void* y;
+    int32_t n, h, w;
+    int32_t ldx, ldy, ldr;
+    int32_t mode; /* enum sfb_c64_mode */
+    int32_t relu;
+    int32_t dtype;
+} sfb_conv_c64_params;
+
+int sfb_conv3x3_c64(const sfb_conv_c64_params* p, sfb_stream_t stream);
+
 /* dst[n, c, hw] (NCHW contiguous) = scale[i] * src[n, hw, c] (NHWC, channel pitch ld_src) for item i,
  * fp32 arithmetic, up to 16 tensors per launch (the ControlNet's down / mid residuals times
  * conditioning_scale).  `scale` is a DEVICE fp32 array [count]: a captured graph serves every scale. */

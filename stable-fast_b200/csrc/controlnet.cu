@@ -1,5 +1,6 @@
 // ControlNet edges: the conditioning embedding's few-channel 3x3 convolutions at image resolution
-// (sfb_conv3x3_small) and the gather of the 13 scaled residuals into the NCHW outputs
+// (sfb_conv3x3_small; sfb_conv3x3_small_ex adds the input transform and ReLU of the tiny VAE's edge
+// convolutions) and the gather of the 13 scaled residuals into the NCHW outputs
 // (sfb_nhwc_to_nchw_scaled).  The reference leaves the whole ControlNetModel to eager PyTorch.
 #include "common.cuh"
 #include "host.h"
@@ -22,7 +23,16 @@ struct ConvSmallArgs {
     const float* bias;
     uint16_t* y;
     int n, h, wd, cin, cin16, cout, stride, ldx, ldy, x_nchw, silu, ho, wo, tiles_w;
+    int in_xform, relu;  // sfb_conv3x3_small_ex (NCHW input only)
 };
+
+// SFB_XFORM_* of an in-image input value, rounded back to 16 bits (the stored input of the conv)
+template <int BF16>
+__device__ __forceinline__ uint16_t xform16(uint16_t v, int xform) {
+    float f = unpack2(v, BF16).x;
+    f = xform == SFB_XFORM_TANH3 ? tanhf(f * (1.0f / 3.0f)) * 3.0f : (f + 1.0f) * 0.5f;
+    return (uint16_t)(pack2(f, 0.f, BF16) & 0xffffu);
+}
 
 template <int BF16>
 __device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -59,6 +69,7 @@ __global__ void __launch_bounds__(128) conv3x3_small_kernel(const ConvSmallArgs 
             uint16_t v = 0;
             if (c < a.cin && gy >= 0 && gy < a.h && gx >= 0 && gx < a.wd)
                 v = a.x[(((size_t)img * a.cin + c) * a.h + gy) * a.wd + gx];
+            if (a.in_xform && c < a.cin && gy >= 0 && gy < a.h && gx >= 0 && gx < a.wd) v = xform16<BF16>(v, a.in_xform);
             halo[(hy * hw + hx) * ps + c] = v;
         }
     } else {
@@ -131,6 +142,7 @@ __global__ void __launch_bounds__(128) conv3x3_small_kernel(const ConvSmallArgs 
                     if (ox >= a.wo) continue;
                     float v0 = acc[mt][nt][2 * half] + b0, v1 = acc[mt][nt][2 * half + 1] + b1;
                     if (a.silu) { v0 = silu_f(v0); v1 = silu_f(v1); }
+                    if (a.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
                     *reinterpret_cast<uint32_t*>(a.y + (((size_t)img * a.ho + oy) * a.wo + ox) * a.ldy + c) =
                         pack2(v0, v1, BF16);
                 }
@@ -188,7 +200,7 @@ __global__ void __launch_bounds__(256) nhwc_to_nchw_scaled_kernel(const NchwScal
 
 using namespace sfb;
 
-extern "C" int sfb_conv3x3_small(const sfb_conv_small_params* p, sfb_stream_t stream) {
+static int conv3x3_small(const sfb_conv_small_params* p, int in_xform, int relu, sfb_stream_t stream) {
     if (!p || !p->x || !p->weight || !p->y || p->n <= 0 || p->h <= 0 || p->w <= 0)
         return fail(SFB_ERR_INVALID, "conv3x3_small: null pointer or empty image");
     if (p->stride != 1 && p->stride != 2) return fail(SFB_ERR_INVALID, "conv3x3_small: stride %d must be 1 or 2", p->stride);
@@ -206,6 +218,7 @@ extern "C" int sfb_conv3x3_small(const sfb_conv_small_params* p, sfb_stream_t st
     a.n = p->n; a.h = p->h; a.wd = p->w; a.cin = p->cin; a.cin16 = (p->cin + 15) / 16 * 16;
     a.cout = p->cout; a.stride = p->stride; a.ldx = p->ldx; a.ldy = p->ldy;
     a.x_nchw = p->x_nchw ? 1 : 0; a.silu = p->silu ? 1 : 0;
+    a.in_xform = in_xform; a.relu = relu ? 1 : 0;
     a.ho = (p->h - 1) / p->stride + 1;
     a.wo = (p->w - 1) / p->stride + 1;
     a.tiles_w = (a.wo + kSmallTW - 1) / kSmallTW;
@@ -232,6 +245,20 @@ extern "C" int sfb_conv3x3_small(const sfb_conv_small_params* p, sfb_stream_t st
         : launch_pdl(conv3x3_small_kernel<0>, grid, dim3(128), smem, static_cast<cudaStream_t>(stream), a);
     if (err != cudaSuccess) return fail(SFB_ERR_CUDA, "conv3x3_small: %s", cudaGetErrorString(err));
     return check_launch("sfb_conv3x3_small");
+}
+
+extern "C" int sfb_conv3x3_small(const sfb_conv_small_params* p, sfb_stream_t stream) {
+    return conv3x3_small(p, SFB_XFORM_NONE, 0, stream);
+}
+
+extern "C" int sfb_conv3x3_small_ex(const sfb_conv_small_ex_params* p, sfb_stream_t stream) {
+    if (!p) return fail(SFB_ERR_INVALID, "conv3x3_small_ex: null params");
+    if (p->in_xform < SFB_XFORM_NONE || p->in_xform > SFB_XFORM_UNIT)
+        return fail(SFB_ERR_INVALID, "conv3x3_small_ex: in_xform %d", p->in_xform);
+    if (p->in_xform != SFB_XFORM_NONE && !p->base.x_nchw)
+        return fail(SFB_ERR_INVALID, "conv3x3_small_ex: an input transform needs the NCHW input (x_nchw = 1)");
+    if (p->relu && p->base.silu) return fail(SFB_ERR_INVALID, "conv3x3_small_ex: relu and silu are exclusive");
+    return conv3x3_small(&p->base, p->in_xform, p->relu, stream);
 }
 
 extern "C" int sfb_nhwc_to_nchw_scaled(const sfb_nhwc_to_nchw_params* p, sfb_stream_t stream) {

@@ -165,7 +165,11 @@ def compile_vae(m, config):
     ``decode(z, num_frames, return_dict=True)``: z holds z.shape[0] / num_frames videos, one launch
     plan and CUDA graph per (frames, num_frames, latent size, dtype), so the pipeline's chunks of
     `decode_chunk_size` frames and its shorter last chunk each get their own.  Another VAE without
-    post_quant_conv, or one missing any parameter of that decoder, keeps its own decode.  fp32 calls
+    post_quant_conv, or one missing any parameter of that decoder, keeps its own decode.  diffusers'
+    AutoencoderTiny (TAESD / TAESDXL) gets the native ``decode(x, generator=None, return_dict=True)`` and
+    ``encode(x, return_dict=True)`` (one plan and CUDA graph per (kind, batch, size, dtype); `use_slicing`
+    runs the whole batch in one plan, `use_tiling` stays on the module's own methods); a tiny VAE whose
+    config the native path does not compute (e.g. 16-channel latents) stays eager with a warning.  fp32 calls
     (force_upcast) and diffusers' tiled encode stay on the module's eager path.  A VAE without a `decode` method is returned unchanged
     with a warning (the reference, too, only hooks what it can trace)."""
     from sfast_b200.runtime import compile_vae_module, require_sm90

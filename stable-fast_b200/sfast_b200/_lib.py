@@ -17,6 +17,8 @@ A_MATRIX, A_CONV3X3, A_UPCONV2X, A_CONV3X1, A_CONV3X3_GN, A_DOWNCONV3X3 = 0, 1, 
 ROW_IDX_DIV_MOD, ROW_IDX_TEMPORAL_CTX = 0, 1
 EPI_STORE, EPI_GEGLU, EPI_QKV, EPI_STORE_F32 = 0, 1, 2, 3
 ACT_NONE, ACT_QUICK_GELU, ACT_GELU, ACT_SILU = 0, 1, 2, 3
+XFORM_NONE, XFORM_TANH3, XFORM_UNIT = 0, 1, 2
+C64_SAME, C64_STRIDE2, C64_UP2X = 0, 1, 2
 
 
 class GemmParams(C.Structure):
@@ -125,6 +127,17 @@ class ConvSmallParams(C.Structure):
                 ("silu", C.c_int32), ("dtype", C.c_int32)]
 
 
+class ConvSmallExParams(C.Structure):
+    _fields_ = [("base", ConvSmallParams), ("in_xform", C.c_int32), ("relu", C.c_int32)]
+
+
+class ConvC64Params(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("weight", C.c_void_p), ("bias", C.c_void_p), ("residual", C.c_void_p),
+                ("y", C.c_void_p), ("n", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("ldx", C.c_int32),
+                ("ldy", C.c_int32), ("ldr", C.c_int32), ("mode", C.c_int32), ("relu", C.c_int32),
+                ("dtype", C.c_int32)]
+
+
 class NchwScaledItem(C.Structure):
     _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("n", C.c_int32), ("c", C.c_int32),
                 ("hw", C.c_int32), ("ld_src", C.c_int32)]
@@ -186,6 +199,8 @@ SYMBOLS = {
     "sfb_clip_pool": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _I32, _I32, _I32, _VP]),
     "sfb_patchify": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "sfb_conv3x3_small": (C.c_int, [C.POINTER(ConvSmallParams), _VP]),
+    "sfb_conv3x3_small_ex": (C.c_int, [C.POINTER(ConvSmallExParams), _VP]),
+    "sfb_conv3x3_c64": (C.c_int, [C.POINTER(ConvC64Params), _VP]),
     "sfb_nhwc_to_nchw_scaled": (C.c_int, [C.POINTER(NhwcToNchwParams), _VP]),
     "sfb_lora_merge": (C.c_int, [C.POINTER(LoraMergeParams), _VP]),
 }

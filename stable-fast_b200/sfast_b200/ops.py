@@ -493,6 +493,48 @@ def conv_small_op(name, lib, *, x, weight, bias, y: Act, n, h, w, cin, cout, str
               2 * n * ho * wo * cout * 9 * cin, 2 * (n * h * w * cin + n * ho * wo * cout))
 
 
+def conv_small_ex_op(name, lib, *, x, weight, bias, y: Act, n, h, w, cin, cout, dt, in_xform=0, relu=False):
+    """sfb_conv3x3_small_ex: stride-1 3x3 pad-1 conv of the NCHW few-channel tensor `x` with the input transform
+    `in_xform` (_lib.XFORM_*) on in-image values and an optional ReLU, into the NHWC activation y; `weight` packed
+    by PackedWeights.conv3x3_small."""
+    p = _lib.ConvSmallExParams()
+    b = p.base
+    b.x, b.weight, b.bias, b.y = _ptr(x), _ptr(weight), _ptr(bias), y.ptr
+    b.n, b.h, b.w, b.cin, b.cout, b.stride = n, h, w, cin, cout, 1
+    b.ldx, b.ldy, b.x_nchw, b.silu, b.dtype = 0, y.ld, 1, 0, dtype_code(dt)
+    p.in_xform, p.relu = in_xform, int(bool(relu))
+    return Op(name, lib.sfb_conv3x3_small_ex, (C.byref(p),), (p, x, weight, bias, y.buf),
+              2 * n * h * w * cout * 9 * cin, 2 * (n * h * w * cin + n * h * w * cout))
+
+
+def c64_out_hw(mode, h, w):
+    """Output size of sfb_conv3x3_c64 in `mode` (_lib.C64_*) for an h x w input."""
+    if mode == _lib.C64_STRIDE2:
+        return (h + 1) // 2, (w + 1) // 2
+    if mode == _lib.C64_UP2X:
+        return 2 * h, 2 * w
+    return h, w
+
+
+def conv_c64_op(name, lib, *, x: Act, weight, bias, y: Act, mode, dt, relu=False, residual: Act = None):
+    """sfb_conv3x3_c64: y = relu?(conv3x3(x) + bias (+ residual)) with 64 input and output channels; `mode`
+    (_lib.C64_*) picks stride 1, stride 2 or nearest-2x upsample first; `weight` packed like
+    PackedWeights.conv3x3_plain ([64, 576]); `bias` fp32 [64] or None."""
+    assert x.c == y.c == 64 and (residual is None or residual.c == 64), (x.c, y.c)
+    if (y.n, y.h, y.w) != (x.n,) + c64_out_hw(mode, x.h, x.w):
+        raise ValueError(f"{name}: output {y.n}x{y.h}x{y.w} does not match mode {mode} of a {x.n}x{x.h}x{x.w} input")
+    p = _lib.ConvC64Params()
+    p.x, p.weight, p.bias, p.y = x.ptr, _ptr(weight), _ptr(bias), y.ptr
+    p.residual = residual.ptr if residual is not None else None
+    p.n, p.h, p.w = x.n, x.h, x.w
+    p.ldx, p.ldy, p.ldr = x.ld, y.ld, residual.ld if residual is not None else 0
+    p.mode, p.relu, p.dtype = mode, int(bool(relu)), dtype_code(dt)
+    nbytes = 2 * 64 * (x.rows + y.rows * (2 if residual is not None else 1))
+    return Op(name, lib.sfb_conv3x3_c64, (C.byref(p),),
+              (p, x.buf, weight, bias, residual.buf if residual is not None else None, y.buf),
+              2 * y.rows * 64 * 9 * 64, nbytes)
+
+
 def conv_out_temporal_op(name, lib, *, x: Act, w, bias, wt, bt, out, frames, dt):
     """sfb_conv_out_temporal: NCHW out [n, cout, H, W] = time_conv_out(conv_out(x)) over videos of `frames`
     frames; `w` packed like PackedWeights.conv3x3_plain, `wt` like PackedWeights.time_conv_out."""

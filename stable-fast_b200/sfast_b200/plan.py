@@ -155,6 +155,15 @@ class PackedWeights:
             return ops.pack_conv3x3(w, self.dtype), b.float().contiguous()
         return self._get(("c3pw", conv, pointwise), build)
 
+    def conv3x3_affine(self, conv, scale, shift):
+        """3x3 conv `conv` (module prefix) followed by y * scale + shift, as one conv: (weight packed like
+        conv3x3_plain of scale * W, fp32 scale * b + shift), formed in fp32 before the weight is rounded."""
+        def build():
+            w = self._raw(conv + ".weight").to(self.device).float() * scale
+            b = self._raw(conv + ".bias").to(self.device).float() * scale + shift
+            return ops.pack_conv3x3(w, self.dtype), b.contiguous()
+        return self._get(("c3aff", conv, scale, shift), build)
+
     def _padded_mat(self, w, kpad):
         """[n, k] weight zero-padded along K to kpad columns, as a GEMM operand."""
         if w.device.type == "meta":

@@ -553,6 +553,101 @@ class CompiledVAE(_CompiledModule):
         return out_cls(latent_dist=dist)
 
 
+class AutoencoderTinyOutput(dict):
+    """Stand-in for diffusers' AutoencoderTinyOutput (attribute, key and index access)."""
+
+    def __init__(self, latents):
+        super().__init__(latents=latents)
+        self.latents = latents
+
+    def __getitem__(self, k):
+        return tuple(self.values())[k] if isinstance(k, int) else super().__getitem__(k)
+
+
+def _tiny_output_class():
+    try:
+        from diffusers.models.autoencoders.autoencoder_tiny import AutoencoderTinyOutput as Out  # type: ignore
+        return Out
+    except Exception:  # noqa: BLE001
+        return AutoencoderTinyOutput
+
+
+def is_tiny_vae(m):
+    """True for a diffusers AutoencoderTiny (TAESD), recognised by its config."""
+    cfg = getattr(m, "config", None)
+    return any(cfg_get(cfg, k) is not None for k in ("decoder_block_out_channels", "num_decoder_blocks"))
+
+
+class CompiledTinyVAE(CompiledVAE):
+    """`AutoencoderTiny.decode(x, generator=None, return_dict=True)` and `encode(x, return_dict=True)` on the
+    native path, sharing one packed copy of the weights and one plan + CUDA-graph cache keyed by
+    (kind, B, H, W, dtype, device).  fp32 calls and `use_tiling` (diffusers' blended tiles: different numbers
+    from a whole-image pass) go to the module's own methods.  `use_slicing` runs the whole batch in one plan:
+    the images are independent, so the result is the per-image one."""
+
+    _what = "tiny VAE"
+
+    def __init__(self, module, enable_cuda_graph=True):
+        from .taesd_plan import taesd_spec_from_config
+        _CompiledModule.__init__(self, taesd_spec_from_config(module.config), module.state_dict, enable_cuda_graph)
+        self._module = module
+        self._eager, self._eager_encode = module.decode, module.encode
+
+    def _eager_reason(self, x):
+        if x.dtype not in (torch.float16, torch.bfloat16):
+            return f"{x.dtype} input: the native path computes in fp16 / bf16"
+        if getattr(self._module, "use_tiling", False):
+            return "use_tiling: diffusers' blended tiles"
+        return None
+
+    def _check(self, x, channels, what):
+        if x.dim() != 4 or x.shape[1] != channels:
+            raise ValueError(f"AutoencoderTiny.{what} of a {tuple(x.shape)} tensor: expected [B, {channels}, H, W]")
+        require_sm90(x.device)
+
+    def decode(self, x, generator=None, return_dict=True):
+        from .taesd_plan import TAESDDecodePlan
+        why = self._eager_reason(x)
+        if why:
+            self._warn_once("decode_eager", "sfast (H100 build): tiny VAE decode left on the module's eager path (%s)",
+                            why)
+            return self._eager(x, generator=generator, return_dict=return_dict)
+        self._check(x, self.spec.latent_channels, "decode")
+        return self._decoder_output(self._step("decode", TAESDDecodePlan, "z_in", x), return_dict)
+
+    def encode(self, x, return_dict=True):
+        from .taesd_plan import TAESDEncodePlan
+        why = self._eager_reason(x)
+        if why:
+            self._warn_once("encode_eager", "sfast (H100 build): tiny VAE encode left on the module's eager path (%s)",
+                            why)
+            return self._eager_encode(x, return_dict=return_dict)
+        self._check(x, self.spec.in_channels, "encode")
+        out = self._step("encode", TAESDEncodePlan, "x_in", x)
+        if not return_dict:
+            return (out,)
+        return _tiny_output_class()(latents=out)
+
+
+def _compile_tiny_vae_module(m, enable_cuda_graph):
+    """Install the native decode and encode of an AutoencoderTiny; None when its config is not supported."""
+    from .taesd_plan import taesd_spec_from_config
+    try:
+        taesd_spec_from_config(m.config)
+    except NotImplementedError as exc:
+        logger.warning("sfast (H100 build): %s: %s", type(m).__name__, exc)
+        return None
+    compiled = CompiledTinyVAE(m, enable_cuda_graph)
+
+    def decode(x, generator=None, return_dict=True):
+        return compiled.decode(x, generator=generator, return_dict=return_dict)
+
+    def encode(x, return_dict=True):
+        return compiled.encode(x, return_dict=return_dict)
+    _install(m, "decode", compiled, decode)
+    return _install(m, "encode", compiled, encode)
+
+
 def _has_temporal_decoder(m):
     """True when m's state dict holds every parameter of SVD's temporal decoder with its shape."""
     from .vae_plan import vae_spec_from_config, vae_temporal_decoder_param_shapes
@@ -568,9 +663,15 @@ def compile_vae_module(m, enable_cuda_graph=True):
     """Replace ``m.decode`` and ``m.encode`` of an AutoencoderKL (same module object).  `encode` is
     replaced only where the module has one and its encoder is supported.  A VAE whose decoder is not the
     2-D one gets the native `decode(z, num_frames, return_dict=True)` of SVD's temporal decoder when its
-    state dict holds every parameter of that decoder; otherwise its decode is kept.  Either entry left
-    alone is logged once."""
+    state dict holds every parameter of that decoder; otherwise its decode is kept.  A tiny VAE
+    (AutoencoderTiny, recognised by its config) gets the native `decode(x, generator=None, return_dict=True)`
+    and `encode(x, return_dict=True)` when its config is supported; otherwise it takes the path below, which
+    leaves both entries alone.  Either entry left alone is logged once."""
     from .vae_plan import vae_encoder_spec_from_config
+    if is_tiny_vae(m) and hasattr(m, "encode"):
+        tiny = _compile_tiny_vae_module(m, enable_cuda_graph)
+        if tiny is not None:
+            return tiny
     eager_decode, temporal = m.decode, False
     if temporal_decoder(m.state_dict()):
         temporal = _has_temporal_decoder(m)

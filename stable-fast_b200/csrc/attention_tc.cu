@@ -474,7 +474,8 @@ static int attention_dispatch(const sfb_attn_params* p, const sfb_attn_ip_params
     if (!p || !p->tmap_q || !p->tmap_k || !p->tmap_vt || !p->out)
         return fail(SFB_ERR_INVALID, "%s: null argument", what);
     if (p->head_dim % 8 || p->head_dim <= 0 || p->seq_q <= 0 || p->seq_kv <= 0)
-        return fail(SFB_ERR_INVALID, "%s: bad geometry", what);
+        return fail(SFB_ERR_INVALID, "%s: bad geometry head_dim=%d seq_q=%d seq_kv=%d", what, p->head_dim, p->seq_q,
+                    p->seq_kv);
     // V^T carries one extra all-ones row at index head_dim (softmax denominator on the tensor
     // core), so its row count is (head_dim + 1) rounded up to 16
     const int dv = (p->head_dim + 1 + 15) / 16 * 16;

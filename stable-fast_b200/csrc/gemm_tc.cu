@@ -1183,6 +1183,11 @@ extern "C" int sfb_gemm(const sfb_gemm_params* p, sfb_stream_t stream_) {
     }
     if (p->rowbias && p->a_mode != SFB_A_CONV3X3 && !tconv && !gnconv)
         return fail(SFB_ERR_INVALID, "sfb_gemm: rowbias (time-embedding add) needs conv mode");
+    // the epilogues read rows of 8 row-bias floats as two float4 loads (global memory when a tile spans more
+    // images than the shared-memory bias slots hold, and in the split-K reduction)
+    if (p->rowbias && ((reinterpret_cast<uintptr_t>(p->rowbias) & 15) || p->ld_rowbias % 4 || p->ld_rowbias < p->N))
+        return fail(SFB_ERR_INVALID, "sfb_gemm: rowbias must be 16-byte aligned with ld_rowbias %% 4 == 0 and "
+                                     ">= N (ld_rowbias=%d)", p->ld_rowbias);
     if (tconv && p->conv_stride != 1) return fail(SFB_ERR_INVALID, "sfb_gemm: temporal conv needs stride 1");
     EpiArgs& e = a.e;
     e.epi = p->epi; e.dtype = p->dtype; e.M = p->M; e.N = p->N;
@@ -1251,6 +1256,8 @@ extern "C" int sfb_gemm(const sfb_gemm_params* p, sfb_stream_t stream_) {
     constexpr int kMaxGridY = 65534;
     if (m_tiles > kMaxGridY && a.splits != 1)
         return fail(SFB_ERR_INVALID, "sfb_gemm: %d M tiles with split-K (at most %d)", m_tiles, kMaxGridY);
+    if (p->defer_finish && a.splits > 1 && (e.epi != SFB_EPI_STORE || e.rowstats_out || e.ln_rowstats))
+        return fail(SFB_ERR_INVALID, "sfb_gemm: defer_finish needs a plain STORE epilogue");
     int rc = 0;
     for (int m0 = 0; m0 < m_tiles && rc == 0; m0 += kMaxGridY) {
         a.m_tile_base = m0;
@@ -1263,11 +1270,7 @@ extern "C" int sfb_gemm(const sfb_gemm_params* p, sfb_stream_t stream_) {
                                      : launch_gemm_t<kGemmStages, 0>(ta, tb, a, grid, stream);
     }
     if (rc) return rc;
-    if (p->defer_finish && a.splits > 1) {
-        if (e.epi != SFB_EPI_STORE || e.rowstats_out || e.ln_rowstats)
-            return fail(SFB_ERR_INVALID, "sfb_gemm: defer_finish needs a plain STORE epilogue");
-        return rc;  // the consumer (sfb_group_norm_fused with part_ws) finishes the tensor
-    }
+    if (p->defer_finish && a.splits > 1) return rc;  // the consumer (sfb_group_norm_fused with part_ws) finishes the tensor
     if (a.splits > 1) {
         const int ncols = (e.epi == SFB_EPI_GEGLU) ? e.geglu_n_out : e.N;
         const long long items = (long long)e.M * (ncols / 8);

@@ -88,7 +88,8 @@ __global__ void __launch_bounds__(256) small_linear_kernel(const SmallLinearArgs
         for (int b = 0; b < nb; ++b) {
             float v = acc[b] + (a.bias ? a.bias[col] : 0.f);
             const size_t o = (size_t)(b0 + b) * a.ldy + col;
-            if (a.add16) v += load1(a.add16, o, a.dtype);
+            // add16 is a contiguous [batch, n] tensor (sfb200.h), not laid out at the output pitch
+            if (a.add16) v += load1(a.add16, (size_t)(b0 + b) * a.n + col, a.dtype);
             if (a.act_out) v = silu_f(v);
             if (a.y32) a.y32[o] = v;
             if (a.y16) store1(a.y16, o, v, a.dtype);
@@ -589,7 +590,10 @@ extern "C" int sfb_copy2d(const void* src, void* dst, int32_t rows, int32_t cols
 extern "C" int sfb_timestep_embed(const float* t, int32_t batch, int32_t dim, int32_t flip,
                                   float freq_shift, void* out, int32_t ldo, int32_t dtype,
                                   sfb_stream_t stream) {
-    if (!t || !out || dim % 2 || batch <= 0) return fail(SFB_ERR_INVALID, "timestep_embed: bad argument");
+    if (!t || !out) return fail(SFB_ERR_INVALID, "timestep_embed: null argument");
+    if (dim <= 0 || dim % 2 || batch <= 0 || ldo < dim)
+        return fail(SFB_ERR_INVALID, "timestep_embed: dim=%d must be even and positive, batch=%d positive, ldo=%d >= dim",
+                    dim, batch, ldo);
     const int half = dim / 2;
     const int total = batch * half;
     cudaError_t err = launch_pdl(timestep_embed_kernel, dim3((total + 127) / 128), dim3(128), 0,
@@ -601,7 +605,9 @@ extern "C" int sfb_timestep_embed(const float* t, int32_t batch, int32_t dim, in
 
 extern "C" int sfb_small_linear(const sfb_small_linear_params* p, sfb_stream_t stream) {
     if (!p || !p->x || !p->w || (!p->y16 && !p->y32)) return fail(SFB_ERR_INVALID, "small_linear: null argument");
-    if (p->k % 8 || p->ldx % 8 || p->batch <= 0 || p->n <= 0) return fail(SFB_ERR_INVALID, "small_linear: k/ldx must be multiples of 8");
+    if (p->k % 8 || p->ldx % 8 || p->batch <= 0 || p->n <= 0)
+        return fail(SFB_ERR_INVALID, "small_linear: k=%d and ldx=%d must be multiples of 8 (batch=%d n=%d)", p->k,
+                    p->ldx, p->batch, p->n);
     SmallLinearArgs a{};
     a.x = reinterpret_cast<const uint16_t*>(p->x);
     a.w = reinterpret_cast<const uint16_t*>(p->w);

@@ -705,7 +705,9 @@ __global__ void __launch_bounds__(256) layer_norm_kernel(const LnArgs a) {
 
 static int make_gn_args(const sfb_gn_params* p, GnArgs& a, int& blocks_per_img) {
     if (!p || !p->x || !p->stats) return fail(SFB_ERR_INVALID, "group_norm: null argument");
-    if (p->c % 8 || p->ldx % 8 || p->groups <= 0 || p->groups > 64 || p->c % p->groups ||
+    // n and hw divide the grid sizing below (an empty tensor has nothing to normalise)
+    if (p->n <= 0 || p->hw <= 0) return fail(SFB_ERR_INVALID, "group_norm: n=%d and hw=%d must be positive", p->n, p->hw);
+    if (p->c <= 0 || p->c % 8 || p->ldx % 8 || p->groups <= 0 || p->groups > 64 || p->c % p->groups ||
         p->c / 8 > kGnThreads || p->c > 4096)
         return fail(SFB_ERR_INVALID, "group_norm: unsupported geometry c=%d groups=%d ldx=%d", p->c, p->groups, p->ldx);
     a.x = reinterpret_cast<const uint16_t*>(p->x);
@@ -872,7 +874,7 @@ extern "C" int sfb_group_norm_fused(const sfb_gn_params* p, sfb_stream_t stream)
 
 extern "C" int sfb_layer_norm(const sfb_ln_params* p, sfb_stream_t stream) {
     if (!p || !p->x || !p->y || !p->gamma || !p->beta) return fail(SFB_ERR_INVALID, "layer_norm: null argument");
-    if (p->c % 8 || p->c > kLnMaxVec * 256 || p->ldx % 8 || p->ldy % 8 || p->rows <= 0)
+    if (p->c <= 0 || p->c % 8 || p->c > kLnMaxVec * 256 || p->ldx % 8 || p->ldy % 8 || p->rows <= 0)
         return fail(SFB_ERR_INVALID, "layer_norm: unsupported geometry c=%d", p->c);
     LnArgs a{};
     a.x = reinterpret_cast<const uint16_t*>(p->x);

@@ -130,7 +130,7 @@ enum sfb_epilogue {
 };
 
 enum { SFB_ACT_NONE = 0, SFB_ACT_QUICK_GELU = 1 /* x * sigmoid(1.702 x) */, SFB_ACT_GELU = 2 /* erf form */,
-       SFB_ACT_SILU = 3 /* x * sigmoid(x) */ };
+       SFB_ACT_SILU = 3 /* x * sigmoid(x) */, SFB_ACT_RELU = 4 /* max(x, 0) */ };
 
 typedef struct sfb_gemm_params {
     const void* tmap_a; /* host pointer to a 128-byte tensor map */
@@ -206,7 +206,8 @@ typedef struct sfb_gemm_params {
     int32_t ln_dim;
     /* element-wise activation of the SFB_EPI_STORE epilogue, applied after bias / LayerNorm fold and
      * before the residual add (the CLIP text encoders' MLP: fc1 + quick_gelu / gelu, encoders traced by
-     * /root/reference/src/sfast/compilers/diffusion_pipeline_compiler.py:93-103).  Needs splits == 1. */
+     * /root/reference/src/sfast/compilers/diffusion_pipeline_compiler.py:93-103; ReLU: the T2I-Adapter's
+     * 3x3 convs).  Needs splits == 1. */
     int32_t act; /* SFB_ACT_* */
     int32_t rowstats_out_slots; /* slots per row of rowstats_out (>= sfb_rowstats_slots(N)) */
     int32_t ln_slots;           /* slots per row of ln_rowstats */
@@ -537,6 +538,23 @@ typedef struct sfb_nhwc_to_nchw_params {
 } sfb_nhwc_to_nchw_params;
 
 int sfb_nhwc_to_nchw_scaled(const sfb_nhwc_to_nchw_params* p, sfb_stream_t stream);
+
+/* ---- T2I-Adapter (diffusers T2IAdapter: PixelUnshuffle, convolutions and 2x2 average pools; the
+ * reference traces the UNet with the adapter residuals as inputs and leaves the adapter eager) ---------- */
+
+/* PixelUnshuffle(r) of a 16-bit NCHW tensor into NHWC:
+ *   y[img, oy, ox, ch * r * r + i * r + j] = x[img, ch, oy * r + i, ox * r + j]
+ * x: NCHW [n, c, h, w] contiguous; y: NHWC [n, h / r, w / r] with channel pitch ldy >= c * r * r (channels
+ * past c * r * r are not written).  r >= 1 divides h and w.  Bit-exact (a permutation). */
+int sfb_pixel_unshuffle(const void* x, void* y, int32_t n, int32_t c, int32_t h, int32_t w, int32_t r,
+                        int32_t ldy, sfb_stream_t stream);
+
+/* nn.AvgPool2d(2, 2) of a 16-bit NHWC tensor: y[img, oy, ox, :] = mean of the 2x2 window at (2oy, 2ox), summed
+ * in fp32 and rounded once.  x: [n, h, w, c] with channel pitch ldx; y: [n, h / 2, w / 2, c] with pitch ldy.
+ * h and w even (where ceil_mode=True pools the same windows); c, ldx, ldy multiples of 8; x and y 16-byte
+ * aligned. */
+int sfb_avg_pool2x2(const void* x, void* y, int32_t n, int32_t h, int32_t w, int32_t c, int32_t ldx,
+                    int32_t ldy, int32_t dtype, sfb_stream_t stream);
 
 /* dst[r, 0:cols] = src[r, 0:cols], 16-bit elements, row pitches in elements */
 int sfb_copy2d(const void* src, void* dst, int32_t rows, int32_t cols, int32_t ld_src,

@@ -84,10 +84,11 @@ struct EpiArgs {
 };
 
 // quick_gelu (x * sigmoid(1.702 x)) / erf gelu of the CLIP text encoders' MLP; SiLU of the ControlNet's
-// conditioning-embedding convs
+// conditioning-embedding convs; ReLU of the T2I-Adapter's 3x3 convs
 __device__ __forceinline__ float epi_act(float x, int act) {
     if (act == SFB_ACT_QUICK_GELU) return __fdividef(x, 1.0f + __expf(-1.702f * x));
     if (act == SFB_ACT_SILU) return silu_f(x);
+    if (act == SFB_ACT_RELU) return fmaxf(x, 0.f);
     return gelu_erf_f(x);
 }
 
@@ -1211,7 +1212,7 @@ extern "C" int sfb_gemm(const sfb_gemm_params* p, sfb_stream_t stream_) {
                         need, p->rowstats_out_slots);
     }
     if (p->ln_rowstats && p->ln_slots < 1) return fail(SFB_ERR_INVALID, "sfb_gemm: ln_rowstats needs ln_slots >= 1");
-    if (p->act < SFB_ACT_NONE || p->act > SFB_ACT_SILU)
+    if (p->act < SFB_ACT_NONE || p->act > SFB_ACT_RELU)
         return fail(SFB_ERR_INVALID, "sfb_gemm: unknown activation %d", p->act);
     if (p->act && (p->epi != SFB_EPI_STORE || p->splits > 1 || p->persistent || p->rowbias))
         return fail(SFB_ERR_INVALID, "sfb_gemm: act needs the STORE epilogue of the one-tile kernel without split-K / row bias");

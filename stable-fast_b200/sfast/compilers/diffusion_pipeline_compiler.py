@@ -53,13 +53,17 @@ def compile(m, config):
     """Compile a diffusers pipeline in place and return it (reference `compile`, :81-124): the UNet, the
     ControlNet (``pipe.controlnet``: a ControlNetModel, or each net of a MultiControlNetModel), the VAE, the
     text encoders and the image encoder run on the native path; a ControlNet class or config the native
-    path does not cover stays eager with a warning.  A loaded IP-Adapter (one plain ``ImageProjection`` or one
+    path does not cover stays eager with a warning.  The T2I-Adapter (``pipe.adapter`` of the adapter pipelines: a
+    T2IAdapter, or each adapter of a MultiAdapter) runs natively too, see `compile_adapter`, and the UNet adds its
+    residuals (``down_intrablock_additional_residuals``) inside its step.  A loaded IP-Adapter (one plain ``ImageProjection`` or one
     IP-Adapter Plus ``IPAdapterPlusImageProjection``) runs inside the UNet's step, see `compile_unet`.  PEFT LoRA
     adapters on the UNet and the text encoders are merged into their packed weights (see `compile_unet`); adapters
     on the ControlNet, the VAE or the vision tower raise ``NotImplementedError`` at their first call."""
     m.unet = compile_unet(m.unet, config)
     if getattr(m, 'controlnet', None) is not None:
         m.controlnet = compile_controlnet(m.controlnet, config)
+    if getattr(m, 'adapter', None) is not None:
+        m.adapter = compile_adapter(m.adapter, config)
     if getattr(m, 'vae', None) is not None:
         m.vae = compile_vae(m.vae, config)
     # text encoders (reference :93-112: lazy trace + CUDA graph of text_encoder / text_encoder_2)
@@ -117,6 +121,39 @@ def compile_controlnet(m, config):
     return _compile_controlnet_net(m, config)
 
 
+def compile_adapter(m, config):
+    """Replace ``m.forward`` of a diffusers T2IAdapter ("full_adapter" or "full_adapter_xl") with the H100-native
+    adapter: one plan and CUDA graph per (batch, image size, dtype); the features are fresh NCHW tensors.  A
+    MultiAdapter (one with ``.adapters``) gets each adapter's forward replaced and keeps its own weighted sum.  Any
+    other class, or a config the native path does not cover (``light_adapter``, channel counts that are not
+    multiples of 64), is left on its eager path with a warning.  The module object is kept, so
+    ``downscale_factor`` and ``total_downscale_factor`` still work."""
+    adapters = getattr(m, 'adapters', None)
+    if adapters is not None:
+        for a in adapters:
+            _compile_adapter_net(a, config)
+        return m
+    return _compile_adapter_net(m, config)
+
+
+def _compile_adapter_net(m, config):
+    from sfast_b200.runtime import compile_adapter_module, require_sm90
+    from sfast_b200.t2i_adapter_plan import t2i_adapter_spec_from_config
+    if type(m).__name__ != 'T2IAdapter' or not hasattr(m, 'config'):
+        logger.warning('sfast (H100 build): %s is not a T2IAdapter; left on its eager path', type(m).__name__)
+        return m
+    try:
+        t2i_adapter_spec_from_config(m.config)
+    except NotImplementedError as exc:
+        logger.warning('sfast (H100 build): T2I-Adapter left on its eager path (%s)', exc)
+        return m
+    device = m.device if hasattr(m, 'device') else torch.device(
+        'cuda' if torch.cuda.is_available() else 'cpu')
+    require_sm90(torch.device(device))
+    return compile_adapter_module(m, enable_cuda_graph=bool(config.enable_cuda_graph),
+                                  preserve_parameters=bool(getattr(config, 'preserve_parameters', True)))
+
+
 def _compile_controlnet_net(m, config):
     from sfast_b200.runtime import compile_controlnet_module, require_sm90
     from sfast_b200.unet_spec import controlnet_spec_from_config
@@ -143,6 +180,12 @@ def compile_unet(m, config):
     over the image features of ``added_cond_kwargs["image_embeds"]``, ``[B, n_img, S_img, D_img]``), runs on
     the step's side stream inside the same CUDA graph, and every cross-attention adds the image-token term.
     FaceID projections, several adapters and ``ip_adapter_masks`` raise ``NotImplementedError`` by name.
+
+    T2I-Adapter residuals (``down_intrablock_additional_residuals``, or diffusers' deprecated form: down residuals
+    without a mid residual) are added where diffusers adds them, one in-place add per insertion point right after
+    the tensor's producer, before any ControlNet residual; a wrong shape raises ``ValueError`` naming the index.
+    Unlike diffusers, the caller's list is not consumed (diffusers pops from it).  Each number of residuals used
+    gets its own plan and CUDA graph; a call without them runs the launch list of a plain step.
 
     PEFT LoRA adapters (diffusers' ``load_lora_weights``), loaded before or after this call, fused or not, are
     merged into the packed weights whenever the adapter state changes (``set_adapters``, ``fuse_lora``,

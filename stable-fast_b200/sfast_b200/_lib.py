@@ -16,7 +16,7 @@ LORA_MAX_ADAPTERS, LORA_MAX_RANK = 8, 256
 A_MATRIX, A_CONV3X3, A_UPCONV2X, A_CONV3X1, A_CONV3X3_GN, A_DOWNCONV3X3 = 0, 1, 2, 3, 4, 5
 ROW_IDX_DIV_MOD, ROW_IDX_TEMPORAL_CTX = 0, 1
 EPI_STORE, EPI_GEGLU, EPI_QKV, EPI_STORE_F32 = 0, 1, 2, 3
-ACT_NONE, ACT_QUICK_GELU, ACT_GELU, ACT_SILU = 0, 1, 2, 3
+ACT_NONE, ACT_QUICK_GELU, ACT_GELU, ACT_SILU, ACT_RELU = 0, 1, 2, 3, 4
 XFORM_NONE, XFORM_TANH3, XFORM_UNIT = 0, 1, 2
 C64_SAME, C64_STRIDE2, C64_UP2X = 0, 1, 2
 
@@ -203,6 +203,8 @@ SYMBOLS = {
     "sfb_conv3x3_c64": (C.c_int, [C.POINTER(ConvC64Params), _VP]),
     "sfb_nhwc_to_nchw_scaled": (C.c_int, [C.POINTER(NhwcToNchwParams), _VP]),
     "sfb_lora_merge": (C.c_int, [C.POINTER(LoraMergeParams), _VP]),
+    "sfb_pixel_unshuffle": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
+    "sfb_avg_pool2x2": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
 }
 
 _lib = None

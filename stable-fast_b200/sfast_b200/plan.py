@@ -31,6 +31,24 @@ def _round_up(a, b):
     return (a + b - 1) // b * b
 
 
+def intrablock_shapes(spec, batch, height, width):
+    """NCHW shapes of the T2I-Adapter residuals (``down_intrablock_additional_residuals``) a 2-D UNet adds, in
+    the order it takes them: one per down block, then one for the mid-block output.  A down block with
+    cross-attention adds its residual to the output of its last (resnet, transformer) pair, in front of its
+    downsampler; a plain down block to its own output, after the downsampler."""
+    out, h, w = [], height, width
+    for blk in spec.down:
+        cross = any(t is not None for t in blk.attentions)
+        if cross:
+            out.append((batch, blk.cout, h, w))
+        if blk.sampler:
+            h, w = h // 2, w // 2
+        if not cross:
+            out.append((batch, blk.cout, h, w))
+    out.append((batch, spec.mid.cout, h, w))
+    return out
+
+
 class PackedWeights:
     """Device-resident, kernel-ready copy of a UNet state dict (shape independent).
 
@@ -678,10 +696,12 @@ class UNetPlan(Plan):
     """One static launch schedule of the UNet for a fixed (batch, height, width)."""
 
     def __init__(self, weights: PackedWeights, batch, height, width, ctx_len=77, controlnet=False, ip_len=0,
-                 ip_seq=0):
+                 ip_seq=0, intrablock=0):
         """`ip_len` > 0: an IP-Adapter (spec.ip) adds ip_len image tokens per sample (n_img images x its
         tokens per image) to every cross-attention; 0 builds exactly the schedule without one.  `ip_seq`:
-        feature tokens per image of an IP-Adapter Plus (spec.ip.resampler), the input of its Resampler."""
+        feature tokens per image of an IP-Adapter Plus (spec.ip.resampler), the input of its Resampler.
+        `intrablock`: how many T2I-Adapter residuals the step adds (the first `intrablock` insertion points of
+        intrablock_shapes, static NCHW inputs `intrablock_in`); 0 builds exactly the schedule without them."""
         spec = weights.spec
         div = 1 << (len(spec.block_out_channels) - 1)
         if height % div or width % div:
@@ -696,6 +716,10 @@ class UNetPlan(Plan):
         self.ctx_len = ctx_len
         self.controlnet = controlnet
         self.ctrl_in = []  # static NCHW inputs: 12 (SD-1.5) down-block residuals + the mid-block one
+        points = intrablock_shapes(spec, batch, height, width)
+        if not 0 <= intrablock <= len(points):
+            raise ValueError(f"intrablock={intrablock}: the UNet has {len(points)} T2I-Adapter insertion points")
+        self.intrablock_in = [self._alloc(s, self.dt) for s in points[:intrablock]]
         # ---- static inputs / output
         self.sample_in = self._alloc((batch, spec.in_channels, height, width), self.dt)
         self.t_in = self._alloc((batch,), torch.float32)
@@ -1029,6 +1053,22 @@ class UNetPlan(Plan):
         else:
             self.conv_in("conv_in", self.sample_in, x)
 
+    def _add_nchw(self, name, srcs, dsts):
+        """dsts[i] (NHWC slices) += srcs[i] (static NCHW inputs) in one sfb_add_nchw_residuals launch."""
+        prm = _lib.AddNchwParams()
+        prm.count, prm.dtype = len(dsts), ops.dtype_code(self.dt)
+        for i, (src, d) in enumerate(zip(srcs, dsts)):
+            it = prm.items[i]
+            it.src, it.dst, it.n, it.c, it.hw, it.ld_dst = _ptr(src), d.ptr, d.n, d.c, d.h * d.w, d.ld
+        self._emit(Op(name, self.lib_or_dry().sfb_add_nchw_residuals, (C.byref(prm),),
+                      (prm, srcs, [d.buf for d in dsts]), 0, sum(3 * t.numel() * 2 for t in srcs)))
+
+    def _intrablock_add(self, i, x: Act):
+        """x += T2I-Adapter residual i, in place, when the step takes one there: right after x's producer, so
+        every later reader (the downsampler, the next block, the up-path skip) sees the sum, as in diffusers."""
+        if i < len(self.intrablock_in):
+            self._add_nchw(f"t2i_adapter.residual.{i}", [self.intrablock_in[i]], [x])
+
     # ------------------------------------------------------------------ whole UNet
     def _build(self):
         spec, B, H, W, lib = self.spec, self.B, self.H, self.W, self.lib_or_dry()
@@ -1068,7 +1108,8 @@ class UNetPlan(Plan):
         self._emit(_JoinOp("temb"))
         # ---- down path
         k = 1
-        for blk in spec.down:
+        for bi, blk in enumerate(spec.down):
+            cross = any(t is not None for t in blk.attentions)
             for r, t in zip(blk.resnets, blk.attentions):
                 dst = skip_dst[k]
                 k += 1
@@ -1079,11 +1120,15 @@ class UNetPlan(Plan):
                     self.resnet(r, x, mid)
                     self.transformer(t, mid, dst)
                 x = dst
+            if cross:
+                self._intrablock_add(bi, x)
             if blk.sampler:
                 dst = skip_dst[k]
                 k += 1
                 self.conv3x3(blk.sampler, x, blk.sampler, dst, stride=2)
                 x = dst
+            if not cross:
+                self._intrablock_add(bi, x)
         # ---- mid
         m = spec.mid
         a = self.act("res_out", x.n, x.h, x.w, m.cout)
@@ -1091,25 +1136,17 @@ class UNetPlan(Plan):
         b = self.act("mid_tf_out", x.n, x.h, x.w, m.cout)
         self.transformer(m.attentions[0], a, b)
         self.resnet(m.resnets[1], b, up_in[(0, 0)][1])
+        self._intrablock_add(len(spec.down), up_in[(0, 0)][1])
         if self.controlnet:
             # ControlNet: skip tensor i += down_block_additional_residuals[i], mid output +=
             # mid_block_additional_residual (diffusers adds them after the down / mid blocks; the
             # reference passes them through its traced UNet as plain inputs,
             # /root/reference/src/sfast/compilers/diffusion_pipeline_compiler.py:89-90).  Every
             # down-path reader of a skip slice has run by now and no up-path reader has: one
-            # multi-tensor launch adds all of them in place.
-            prm = _lib.AddNchwParams()
+            # multi-tensor launch adds all of them in place (on top of any T2I-Adapter residual).
             dsts = [skip_dst[i] for i in range(len(skip_shapes))] + [up_in[(0, 0)][1]]
-            prm.count, prm.dtype = len(dsts), ops.dtype_code(self.dt)
-            for i, d in enumerate(dsts):
-                src = self._alloc((B, d.c, d.h, d.w), self.dt)
-                self.ctrl_in.append(src)
-                it = prm.items[i]
-                it.src, it.dst, it.n, it.c, it.hw, it.ld_dst = _ptr(src), d.ptr, B, d.c, d.h * d.w, d.ld
-            import ctypes
-            self._emit(Op("controlnet.residuals", lib.sfb_add_nchw_residuals, (ctypes.byref(prm),),
-                          (prm, self.ctrl_in, [d.buf for d in dsts]), 0,
-                          sum(3 * t.numel() * 2 for t in self.ctrl_in)))
+            self.ctrl_in = [self._alloc((B, d.c, d.h, d.w), self.dt) for d in dsts]
+            self._add_nchw("controlnet.residuals", self.ctrl_in, dsts)
         # ---- up path
         for i, blk in enumerate(spec.up):
             n_res = len(blk.resnets)

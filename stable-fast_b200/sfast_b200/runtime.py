@@ -16,7 +16,7 @@ import time
 import torch
 
 from . import lora
-from .plan import PackedWeights, UNetPlan
+from .plan import PackedWeights, UNetPlan, intrablock_shapes
 from .svd_plan import SVDPlan
 from .unet_spec import cfg_get, ip_adapter_spec, ip_scale_of, spec_from_config
 
@@ -41,8 +41,14 @@ except Exception:  # noqa: BLE001
             return tuple(self.values())
 
 
-_UNSUPPORTED_KWARGS = ("class_labels", "timestep_cond", "attention_mask",
-                       "down_intrablock_additional_residuals", "encoder_attention_mask")
+_UNSUPPORTED_KWARGS = ("class_labels", "timestep_cond", "attention_mask", "encoder_attention_mask")
+
+
+class LegacyResidualShapeError(ValueError, NotImplementedError):
+    """A residual of diffusers' deprecated T2I-Adapter form (``down_block_additional_residuals`` without
+    ``mid_block_additional_residual``) whose shape fits no insertion point.  Such a list is most likely a
+    ControlNet's down residuals passed without their mid residual, which the UNet refuses: the error is also
+    the NotImplementedError it raised for that call before the T2I-Adapter form was supported."""
 
 
 def require_sm90(device):
@@ -291,6 +297,30 @@ class CompiledUNet(_CompiledModule):
         scales = [ip_scale_of(p, n) for p, n in zip(self._ip_procs, ip.layers)]
         return emb.shape[1] * ip.tokens, ip_seq, emb.reshape(-1, ip.image_embed_dim), scales
 
+    def _intrablock_inputs(self, residuals, B, H, W, legacy):
+        """The T2I-Adapter residuals this call adds, in order: one per down block, then the mid-block one when
+        the next residual has the mid output's shape (diffusers' rule for T2I-Adapter-XL); any further ones are
+        ignored, as diffusers ignores them.  The caller's list is not modified (diffusers pops from it).  Raises
+        ValueError naming the index of a down-block residual whose shape does not fit."""
+        points = intrablock_shapes(self.spec, B, H, W)
+        n_down = len(points) - 1
+        res = list(residuals)
+        arg = "down_block_additional_residuals" if legacy else "down_intrablock_additional_residuals"
+        for i, r in enumerate(res[:n_down]):
+            if tuple(r.shape) != points[i]:
+                msg = (f"{arg}[{i}] has shape {tuple(r.shape)}; down block {i} adds a T2I-Adapter residual of "
+                       f"shape {points[i]}")
+                if legacy:
+                    raise LegacyResidualShapeError(
+                        msg + " (without mid_block_additional_residual this is diffusers' deprecated T2I-Adapter "
+                        "form; ControlNet residuals need both down_block_additional_residuals and "
+                        "mid_block_additional_residual)")
+                raise ValueError(msg)
+        n = min(len(res), n_down)
+        if len(res) > n_down and tuple(res[n_down].shape) == points[n_down]:
+            n += 1
+        return res[:n]
+
     # -- forward -------------------------------------------------------------------------
     def _call_svd(self, sample, timestep, encoder_hidden_states, added_time_ids, return_dict=True):
         """diffusers UNetSpatioTemporalConditionModel.forward(sample [B, F, C, H, W], timestep,
@@ -337,9 +367,7 @@ class CompiledUNet(_CompiledModule):
                  mid_block_additional_residual=None, down_intrablock_additional_residuals=None,
                  encoder_attention_mask=None, return_dict=True):
         given = dict(class_labels=class_labels, timestep_cond=timestep_cond,
-                     attention_mask=attention_mask,
-                     down_intrablock_additional_residuals=down_intrablock_additional_residuals,
-                     encoder_attention_mask=encoder_attention_mask)
+                     attention_mask=attention_mask, encoder_attention_mask=encoder_attention_mask)
         for k in _UNSUPPORTED_KWARGS:
             if given[k] is not None:
                 raise NotImplementedError(f"sfast (H100 build): UNet argument `{k}` is not supported")
@@ -356,18 +384,28 @@ class CompiledUNet(_CompiledModule):
         if dtype not in (torch.float16, torch.bfloat16):
             raise NotImplementedError(f"sfast (H100 build): UNet dtype {dtype}; use fp16 or bf16")
         ctx_len = encoder_hidden_states.shape[1]
+        legacy = (down_intrablock_additional_residuals is None and mid_block_additional_residual is None
+                  and down_block_additional_residuals is not None)
+        if legacy:  # diffusers' deprecated T2I-Adapter form: the down residuals are the adapter's
+            down_intrablock_additional_residuals, down_block_additional_residuals = down_block_additional_residuals, None
         controlnet = down_block_additional_residuals is not None or mid_block_additional_residual is not None
         if controlnet and (down_block_additional_residuals is None or mid_block_additional_residual is None):
             raise NotImplementedError("sfast (H100 build): ControlNet residuals need both "
                                       "down_block_additional_residuals and mid_block_additional_residual")
+        intrablock = []
+        if down_intrablock_additional_residuals is not None:
+            intrablock = self._intrablock_inputs(down_intrablock_additional_residuals, B, H, W, legacy)
         # everything below (allocation, TMA maps, launches, capture) targets sample's device
         with self._lock, torch.cuda.device(sample.device):
             t_first = time.perf_counter() if self.first_call_s is None else None
             weights = self._weights_for(dtype, sample.device, lora_scale)
-            gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index, controlnet, ip_len, ip_seq),
+            gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index, controlnet, ip_len, ip_seq,
+                                len(intrablock)),
                                lambda: UNetPlan(weights, B, H, W, ctx_len, controlnet=controlnet, ip_len=ip_len,
-                                                ip_seq=ip_seq))
+                                                ip_seq=ip_seq, intrablock=len(intrablock)))
             plan = gp.plan
+            for dst, src in zip(plan.intrablock_in, intrablock):
+                dst.copy_(src, non_blocking=True)
             if ip_len:
                 plan.image_embeds_in.copy_(image_embeds, non_blocking=True)
                 plan.ip_scale_in.copy_(torch.tensor(ip_scales, dtype=torch.float32))
@@ -965,6 +1003,47 @@ def compile_controlnet_module(m, enable_cuda_graph=True, preserve_parameters=Tru
 
     def forward(*args, **kwargs):
         return compiled(*args, **kwargs)
+    return _install(m, "forward", compiled, forward)
+
+
+class CompiledT2IAdapter(_CompiledModule):
+    """Callable with the signature of diffusers ``T2IAdapter.forward(x)``: the list of NCHW features, fresh
+    tensors.  One plan + CUDA graph per (batch, image height, width, dtype, device)."""
+
+    _what = "T2I-Adapter"
+
+    def __init__(self, config, state_dict_fn, enable_cuda_graph=True, preserve_parameters=True):
+        from .t2i_adapter_plan import t2i_adapter_spec_from_config
+        super().__init__(t2i_adapter_spec_from_config(config), state_dict_fn, enable_cuda_graph, preserve_parameters)
+
+    def __call__(self, x):
+        from .t2i_adapter_plan import AdapterPlan
+        spec = self.spec
+        if x.dim() != 4 or x.shape[1] != spec.in_channels:
+            raise ValueError(f"T2IAdapter input of shape {tuple(x.shape)}: expected [B, {spec.in_channels}, H, W]")
+        if x.dtype not in (torch.float16, torch.bfloat16):
+            raise NotImplementedError(f"sfast (H100 build): T2I-Adapter dtype {x.dtype}; use fp16 or bf16")
+        B, _, H, W = x.shape
+        f = spec.total_downscale_factor
+        if H % f or W % f:
+            raise NotImplementedError(f"sfast (H100 build): T2I-Adapter image size {H}x{W} must be a multiple of its "
+                                      f"total_downscale_factor {f}")
+        require_sm90(x.device)
+        with self._lock, torch.cuda.device(x.device):
+            weights = self._weights_for(x.dtype, x.device)
+            gp = self._graphed((B, H, W, x.dtype, x.device.index), lambda: AdapterPlan(weights, B, H, W))
+            gp.plan.x_in.copy_(x, non_blocking=True)
+            gp.step()
+            return [o.clone() for o in gp.plan.features_out]
+
+
+def compile_adapter_module(m, enable_cuda_graph=True, preserve_parameters=True):
+    """Replace ``m.forward`` of a diffusers T2IAdapter (same module object: ``downscale_factor`` and
+    ``total_downscale_factor`` keep working)."""
+    compiled = CompiledT2IAdapter(m.config, m.state_dict, enable_cuda_graph, preserve_parameters)
+
+    def forward(x):
+        return compiled(x)
     return _install(m, "forward", compiled, forward)
 
 

@@ -13,9 +13,11 @@ each key once on fresh seeded inputs:
     gamma-folded weights and their column sums);
   * the reference is float64, written from the semantics in include/sfb200.h;
   * every output buffer is filled with a sentinel bit pattern first: pitch gaps, leading offsets and
-    a guard band of GUARD_ROWS rows past the last row must come back bit-for-bit unchanged.
+    a guard band of GUARD_ROWS rows past the last row must come back bit-for-bit unchanged;
+  * optionally (`soundness`), every launch also checks the access model of plan_hazards.py: bytes written
+    outside its write regions, and outputs that depend on bytes outside its read regions, fail the key.
 
-    python tests/plan_launches.py [--plans NAME ...] [--all] [--json out.json] [--list]
+    python tests/plan_launches.py [--plans NAME ...] [--all] [--json out.json] [--list] [--soundness]
 
 prints one JSON line per key (key id, entry point, plans that emit it, error, tolerance, pass) and a
 summary of the largest error per entry point.  Without --all only the default subset
@@ -1335,28 +1337,41 @@ def describe(key):
     return f"{name}({show})"
 
 
-def replay(key, ent, peaked=False):
-    """Replay one key on the GPU: a Result."""
+def replay(key, ent, peaked=False, soundness=None):
+    """Replay one key on the GPU: a Result.  `soundness` "w" / "rw": also check the access model of
+    plan_hazards.py against every launch of the replay -- its writes ("w"), and its writes and reads ("rw")."""
     seed = int(hashlib.sha1(repr(key).encode()).hexdigest()[:8], 16) + int(peaked)
     torch.manual_seed(seed)
     try:
-        return REPLAY[ent["name"]](ent["op"], peaked=peaked)
+        if not soundness:
+            return REPLAY[ent["name"]](ent["op"], peaked=peaked)
+        import plan_hazards  # (imports this module)
+        with plan_hazards.checking_launches(read_check="r" in soundness) as sound:
+            res = REPLAY[ent["name"]](ent["op"], peaked=peaked)
+        assert sound.writes and (sound.reads or "r" not in soundness), "no launch of the replay was checked"
+        res.add("access_model", float("inf") if sound.violations else 0.0, 0.0)
+        res.model = sound.violations
+        return res
     finally:
         torch.cuda.synchronize()
         torch.cuda.empty_cache()
 
 
-def run_keys(entries, keys, log=None):
-    """Replay `keys`; yields one record per replay (peaked entry points twice)."""
+def run_keys(entries, keys, log=None, soundness=None):
+    """Replay `keys`; yields one record per replay (peaked entry points twice).  `soundness`: {key: "w" / "rw"},
+    the access-model check of each key's first replay (replay())."""
     for key in keys:
         ent = entries[key]
         for peaked in ((False, True) if ent["name"] in PEAKED else (False,)):
             t0 = time.time()
+            sound = None if peaked or not soundness else soundness.get(key)
             try:
-                r = replay(key, ent, peaked)
+                r = replay(key, ent, peaked, sound)
                 err, tl = r.main()
                 rec = dict(key=key_id(key), entry=ent["name"], peaked=peaked, desc=describe(key), plans=ent["plans"],
                            err=err, tol=tl, parts=[(w, e, t) for w, e, t in r.parts], ok=r.ok)
+                if sound:
+                    rec.update(soundness=sound, model=getattr(r, "model", []))
             except Exception as e:  # noqa: BLE001  -- a launch the library refuses is a failing key
                 rec = dict(key=key_id(key), entry=ent["name"], peaked=peaked, desc=describe(key), plans=ent["plans"],
                            err=float("inf"), tol=0.0, error=repr(e)[:400], ok=False)
@@ -1384,6 +1399,8 @@ def main(argv=None):
     ap.add_argument("--all", action="store_true", help="replay every distinct key, not the default subset")
     ap.add_argument("--json", help="also write the records (and the summary) to this JSON file")
     ap.add_argument("--list", action="store_true", help="list plans and distinct keys per entry point, no GPU")
+    ap.add_argument("--soundness", action="store_true",
+                    help="also check plan_hazards.py's access model: writes on every key, reads on the default subset")
     args = ap.parse_args(argv)
     t0 = time.time()
     entries, names = collect(args.plans)
@@ -1400,7 +1417,11 @@ def main(argv=None):
         return 0
     torch.cuda.reset_peak_memory_stats()
     t1 = time.time()
-    records = list(run_keys(entries, keys, log=lambda r: print(json.dumps(r), flush=True)))
+    sound = None
+    if args.soundness:
+        sub = set(select_subset(entries))
+        sound = {k: "rw" if k in sub else "w" for k in keys}
+    records = list(run_keys(entries, keys, log=lambda r: print(json.dumps(r), flush=True), soundness=sound))
     summ = summarize(records)
     tail = {"summary": {k: dict(max_err=v[0], tol=v[1], replays=v[2], failures=v[3]) for k, v in sorted(summ.items())},
             "replay_seconds": round(time.time() - t1, 1),

@@ -556,6 +556,25 @@ int sfb_pixel_unshuffle(const void* x, void* y, int32_t n, int32_t c, int32_t h,
 int sfb_avg_pool2x2(const void* x, void* y, int32_t n, int32_t h, int32_t w, int32_t c, int32_t ldx,
                     int32_t ldy, int32_t dtype, sfb_stream_t stream);
 
+/* ---- FreeU (diffusers UNet2DConditionModel.enable_freeu: up blocks 0 and 1 rescale the backbone features and
+ * filter the skip features in front of every resnet; the reference traces the forward, torch.fft included) --- */
+
+/* FreeU on one up-block resnet's NHWC concat buffer x [n, h, w] (channel pitch ld) = hidden [0, c_hidden) |
+ * skip [c_hidden, c_hidden + c_skip), in place, 16-bit:
+ *   hidden channels [0, c_hidden / 2):  y = x * b       (one fp32 multiply, one rounding: torch's x * b)
+ *   skip channels:                      y = diffusers' fourier_filter(x, threshold=1, scale=s) per (image,
+ *                                       channel), computed in closed form in fp32 with one rounding;
+ *   every other channel and the pitch gap are not touched.
+ * bs: DEVICE fp32 [2] = (b, s): a captured graph serves every value.  c_hidden, c_skip and ld are positive
+ * multiples of 8, ld >= c_hidden + c_skip, x 16-byte aligned. */
+typedef struct sfb_freeu_params {
+    void* x;
+    const float* bs;
+    int32_t n, h, w, c_hidden, c_skip, ld, dtype;
+} sfb_freeu_params;
+
+int sfb_freeu(const sfb_freeu_params* p, sfb_stream_t stream);
+
 /* dst[r, 0:cols] = src[r, 0:cols], 16-bit elements, row pitches in elements */
 int sfb_copy2d(const void* src, void* dst, int32_t rows, int32_t cols, int32_t ld_src,
                int32_t ld_dst, sfb_stream_t stream);

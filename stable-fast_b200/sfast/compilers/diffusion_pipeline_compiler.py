@@ -191,7 +191,13 @@ def compile_unet(m, config):
     merged into the packed weights whenever the adapter state changes (``set_adapters``, ``fuse_lora``,
     ``disable_lora``, ``delete_adapters``, ...); ``cross_attention_kwargs={"scale": s}`` scales the active
     adapters for that call.  The step's launch list and CUDA graph are those of the adapter-free UNet.  DoRA,
-    ``lora_bias`` and non-LoRA PEFT adapters raise ``NotImplementedError`` naming the layer."""
+    ``lora_bias`` and non-LoRA PEFT adapters raise ``NotImplementedError`` naming the layer.
+
+    FreeU (``pipe.enable_freeu(s1, s2, b1, b2)`` / ``unet.enable_freeu``) is read from ``up_blocks[0]`` and
+    ``[1]`` on every call, with diffusers' rule per block (on when all four of its values are truthy): the
+    backbone scaling and the Fourier skip filter run natively in front of each resnet of those blocks, inside the
+    CUDA graph.  Each on/off pair gets its own plan; changing the values reuses it, and with FreeU off the step
+    is the plain one."""
     from sfast_b200.runtime import compile_unet_module, require_sm90
     device = m.device if hasattr(m, 'device') else torch.device(
         'cuda' if torch.cuda.is_available() else 'cpu')

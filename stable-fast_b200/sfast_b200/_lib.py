@@ -147,6 +147,11 @@ class NhwcToNchwParams(C.Structure):
     _fields_ = [("count", C.c_int32), ("dtype", C.c_int32), ("scale", C.c_void_p), ("items", NchwScaledItem * 16)]
 
 
+class FreeUParams(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("bs", C.c_void_p), ("n", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
+                ("c_hidden", C.c_int32), ("c_skip", C.c_int32), ("ld", C.c_int32), ("dtype", C.c_int32)]
+
+
 class LoraAdapter(C.Structure):
     _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("rank", C.c_int32), ("lda", C.c_int32), ("ldb", C.c_int32),
                 ("a_dtype", C.c_int32), ("b_dtype", C.c_int32), ("scale", C.c_float)]
@@ -205,6 +210,7 @@ SYMBOLS = {
     "sfb_lora_merge": (C.c_int, [C.POINTER(LoraMergeParams), _VP]),
     "sfb_pixel_unshuffle": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "sfb_avg_pool2x2": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
+    "sfb_freeu": (C.c_int, [C.POINTER(FreeUParams), _VP]),
 }
 
 _lib = None

@@ -696,12 +696,15 @@ class UNetPlan(Plan):
     """One static launch schedule of the UNet for a fixed (batch, height, width)."""
 
     def __init__(self, weights: PackedWeights, batch, height, width, ctx_len=77, controlnet=False, ip_len=0,
-                 ip_seq=0, intrablock=0):
+                 ip_seq=0, intrablock=0, freeu=(False, False)):
         """`ip_len` > 0: an IP-Adapter (spec.ip) adds ip_len image tokens per sample (n_img images x its
         tokens per image) to every cross-attention; 0 builds exactly the schedule without one.  `ip_seq`:
         feature tokens per image of an IP-Adapter Plus (spec.ip.resampler), the input of its Resampler.
         `intrablock`: how many T2I-Adapter residuals the step adds (the first `intrablock` insertion points of
-        intrablock_shapes, static NCHW inputs `intrablock_in`); 0 builds exactly the schedule without them."""
+        intrablock_shapes, static NCHW inputs `intrablock_in`); 0 builds exactly the schedule without them.
+        `freeu`: (up block 0, up block 1) flags; a block that is on runs FreeU (sfb_freeu) in front of each of
+        its resnets with the values of the static input `freeu_in` = (b1, s1, b2, s2); (False, False) builds
+        exactly the schedule without it."""
         spec = weights.spec
         div = 1 << (len(spec.block_out_channels) - 1)
         if height % div or width % div:
@@ -720,6 +723,14 @@ class UNetPlan(Plan):
         if not 0 <= intrablock <= len(points):
             raise ValueError(f"intrablock={intrablock}: the UNet has {len(points)} T2I-Adapter insertion points")
         self.intrablock_in = [self._alloc(s, self.dt) for s in points[:intrablock]]
+        self.freeu = tuple(bool(f) for f in freeu)
+        if len(self.freeu) != 2:
+            raise ValueError(f"freeu={freeu!r}: one flag for each of up blocks 0 and 1")
+        if any(self.freeu):
+            if len(spec.up) < 2:
+                raise ValueError(f"freeu={freeu!r}: the UNet has {len(spec.up)} up blocks")
+            # device memory: a captured graph serves every value
+            self.freeu_in = self._alloc((4,), torch.float32)
         # ---- static inputs / output
         self.sample_in = self._alloc((batch, spec.in_channels, height, width), self.dt)
         self.t_in = self._alloc((batch,), torch.float32)
@@ -1069,6 +1080,17 @@ class UNetPlan(Plan):
         if i < len(self.intrablock_in):
             self._add_nchw(f"t2i_adapter.residual.{i}", [self.intrablock_in[i]], [x])
 
+    def _freeu(self, i, name, cat: Act, c_hidden):
+        """FreeU of up block i (0 or 1) on one resnet's concat buffer `cat` = hidden [0, c_hidden) | skip, in
+        place: after every writer of the buffer and before its resnet, the only reader of both slices."""
+        p = _lib.FreeUParams()
+        p.x, p.bs = cat.ptr, _ptr(self.freeu_in) + 8 * i
+        p.n, p.h, p.w, p.c_hidden, p.c_skip, p.ld = cat.n, cat.h, cat.w, c_hidden, cat.c - c_hidden, cat.ld
+        p.dtype = ops.dtype_code(self.dt)
+        rows = cat.n * cat.h * cat.w
+        self._emit(Op(name, self.lib_or_dry().sfb_freeu, (C.byref(p),), (p, cat.buf, self.freeu_in), 0,
+                      rows * (c_hidden + 3 * p.c_skip) * 2))
+
     # ------------------------------------------------------------------ whole UNet
     def _build(self):
         spec, B, H, W, lib = self.spec, self.B, self.H, self.W, self.lib_or_dry()
@@ -1152,6 +1174,8 @@ class UNetPlan(Plan):
             n_res = len(blk.resnets)
             for j, (r, t) in enumerate(zip(blk.resnets, blk.attentions)):
                 xin = up_in[(i, j)][0]
+                if i < 2 and self.freeu[i]:
+                    self._freeu(i, r.prefix + ".freeu", xin, up_in[(i, j)][1].c)
                 last = j == n_res - 1
                 if not last:
                     dst = up_in[(i, j + 1)][1]

@@ -321,6 +321,24 @@ class CompiledUNet(_CompiledModule):
             n += 1
         return res[:n]
 
+    def _freeu_state(self):
+        """((on0, on1), [b1, s1, b2, s2]) of this call: the FreeU attributes diffusers' ``enable_freeu`` sets on
+        ``up_blocks[0]`` and ``[1]``.  Like diffusers' up blocks, a block applies FreeU only when all four of its
+        own s1, s2, b1, b2 are truthy (so a zero switches it off, and ``disable_freeu`` sets them to None); block 0
+        uses its b1 / s1, block 1 its b2 / s2.  Later up blocks do nothing in diffusers either.  Without the
+        module (compiled from its config alone) FreeU is off."""
+        blocks = getattr(self._module, "up_blocks", None)
+        if blocks is None or len(blocks) < 2:
+            return (False, False), None
+        on = tuple(all(getattr(blk, k, None) for k in ("s1", "s2", "b1", "b2")) for blk in blocks[:2])
+        if not any(on):
+            return on, None
+        vals = [0.0] * 4
+        for i, (b, s) in enumerate((("b1", "s1"), ("b2", "s2"))):
+            if on[i]:
+                vals[2 * i], vals[2 * i + 1] = float(getattr(blocks[i], b)), float(getattr(blocks[i], s))
+        return on, vals
+
     # -- forward -------------------------------------------------------------------------
     def _call_svd(self, sample, timestep, encoder_hidden_states, added_time_ids, return_dict=True):
         """diffusers UNetSpatioTemporalConditionModel.forward(sample [B, F, C, H, W], timestep,
@@ -395,17 +413,20 @@ class CompiledUNet(_CompiledModule):
         intrablock = []
         if down_intrablock_additional_residuals is not None:
             intrablock = self._intrablock_inputs(down_intrablock_additional_residuals, B, H, W, legacy)
+        freeu, freeu_vals = self._freeu_state()
         # everything below (allocation, TMA maps, launches, capture) targets sample's device
         with self._lock, torch.cuda.device(sample.device):
             t_first = time.perf_counter() if self.first_call_s is None else None
             weights = self._weights_for(dtype, sample.device, lora_scale)
-            gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index, controlnet, ip_len, ip_seq,
+            gp = self._graphed((B, H, W, dtype, ctx_len, sample.device.index, controlnet, ip_len, ip_seq, freeu,
                                 len(intrablock)),
                                lambda: UNetPlan(weights, B, H, W, ctx_len, controlnet=controlnet, ip_len=ip_len,
-                                                ip_seq=ip_seq, intrablock=len(intrablock)))
+                                                ip_seq=ip_seq, intrablock=len(intrablock), freeu=freeu))
             plan = gp.plan
             for dst, src in zip(plan.intrablock_in, intrablock):
                 dst.copy_(src, non_blocking=True)
+            if freeu_vals is not None:
+                plan.freeu_in.copy_(torch.tensor(freeu_vals, dtype=torch.float32))
             if ip_len:
                 plan.image_embeds_in.copy_(image_embeds, non_blocking=True)
                 plan.ip_scale_in.copy_(torch.tensor(ip_scales, dtype=torch.float32))

@@ -359,6 +359,11 @@ int sfb_small_linear(const sfb_small_linear_params* p, sfb_stream_t stream);
  * a[p, (kh*3+kw)*cin + c] and zero padding up to 64; feeds sfb_gemm (K = 64). */
 int sfb_im2col_in(const void* x, void* a, int32_t n, int32_t h, int32_t wd, int32_t cin,
                   sfb_stream_t stream);
+/* The same for a wide first convolution (e.g. the inpainting UNets' 9 input channels): x NCHW
+ * [n, 9 <= cin <= 14, h, w] 16-bit -> a [n*h*w, 128] 16-bit with a[p, (kh*3+kw)*cin + c] and zero
+ * padding up to 128; feeds sfb_gemm (K = 128).  n, h, w positive, n*h*w < 2^31. */
+int sfb_im2col_in_wide(const void* x, void* a, int32_t n, int32_t h, int32_t wd, int32_t cin,
+                       sfb_stream_t stream);
 int sfb_conv_in(const void* x, const void* w, const float* bias, void* y, int32_t n, int32_t h,
                 int32_t wd, int32_t cin, int32_t cout, int32_t ldy, int32_t dtype,
                 sfb_stream_t stream);

@@ -211,6 +211,44 @@ __global__ void __launch_bounds__(128) im2col_in_kernel(const uint16_t* __restri
 }
 
 // ---------------------------------------------------------------------------------------
+// im2col for a wide first convolution (9 <= cin <= 14: K = 9*cin <= 126, e.g. the inpainting
+// UNets' 9 channels): NCHW input -> A[pixels, 128] (K zero-padded to two 64-wide K blocks).
+// One thread per output pixel.  Each output column's (tap, ci) is carried along the unrolled
+// column loop, so every register index is a compile-time constant (no local-memory row array).
+// ---------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128) im2col_in_wide_kernel(const uint16_t* __restrict__ x,
+                                                             uint16_t* __restrict__ a, int n, int h, int w,
+                                                             int cin) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n * h * w) return;
+    const int xw = p % w;
+    const int yh = (p / w) % h;
+    const int img = p / (w * h);
+    const size_t plane = (size_t)h * w;
+    const uint16_t* xi = x + (size_t)img * cin * plane;
+    uint4* dst = reinterpret_cast<uint4*>(a + (size_t)p * 128);
+    int tap = 0, ci = 0;
+#pragma unroll
+    for (int v = 0; v < 16; ++v) {
+        uint32_t word[4];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            uint32_t val = 0;
+            if (tap < 9) {
+                const int iy = yh + tap / 3 - 1, ix = xw + tap % 3 - 1;
+                if (iy >= 0 && iy < h && ix >= 0 && ix < w) val = xi[ci * plane + (size_t)iy * w + ix];
+            }
+            if (e & 1) word[e >> 1] |= val << 16;
+            else word[e >> 1] = val;
+            if (++ci == cin) { ci = 0; ++tap; }
+        }
+        dst[v] = make_uint4(word[0], word[1], word[2], word[3]);
+    }
+}
+
+// ---------------------------------------------------------------------------------------
 // conv_out: NHWC (pitch ld) -> NCHW (cout <= 8), 3x3 pad 1.  One warp per output pixel; lanes
 // split the 9 * cin/8 (tap, 8-channel vector) items; weights [cout][9][cin] staged in smem.
 // ---------------------------------------------------------------------------------------
@@ -648,6 +686,23 @@ extern "C" int sfb_im2col_in(const void* x, void* a, int32_t n, int32_t h, int32
                                  reinterpret_cast<uint16_t*>(a), n, h, wd, cin);
     if (err != cudaSuccess) return fail(SFB_ERR_CUDA, "im2col_in: %s", cudaGetErrorString(err));
     return check_launch("sfb_im2col_in");
+}
+
+extern "C" int sfb_im2col_in_wide(const void* x, void* a, int32_t n, int32_t h, int32_t wd, int32_t cin,
+                                  sfb_stream_t stream) {
+    if (!x || !a) return fail(SFB_ERR_INVALID, "im2col_in_wide: null argument");
+    if (reinterpret_cast<uintptr_t>(a) & 15) return fail(SFB_ERR_INVALID, "im2col_in_wide: a must be 16-byte aligned");
+    if (n <= 0 || h <= 0 || wd <= 0) return fail(SFB_ERR_INVALID, "im2col_in_wide: n=%d h=%d w=%d must be positive",
+                                                 n, h, wd);
+    if ((int64_t)n * h * wd > INT32_MAX)
+        return fail(SFB_ERR_INVALID, "im2col_in_wide: n*h*w=%lld must be below 2^31", (long long)n * h * wd);
+    if (cin < 9 || cin > 14) return fail(SFB_ERR_INVALID, "im2col_in_wide: cin=%d must be 9..14", cin);
+    const int total = n * h * wd;
+    cudaError_t err = launch_pdl(im2col_in_wide_kernel, dim3((total + 127) / 128), dim3(128), 0,
+                                 static_cast<cudaStream_t>(stream), reinterpret_cast<const uint16_t*>(x),
+                                 reinterpret_cast<uint16_t*>(a), n, h, wd, cin);
+    if (err != cudaSuccess) return fail(SFB_ERR_CUDA, "im2col_in_wide: %s", cudaGetErrorString(err));
+    return check_launch("sfb_im2col_in_wide");
 }
 
 extern "C" int sfb_conv_out(const void* x, const void* w, const float* bias, void* y, int32_t n,

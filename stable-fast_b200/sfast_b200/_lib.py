@@ -186,6 +186,7 @@ SYMBOLS = {
     "sfb_timestep_embed": (C.c_int, [_VP, _I32, _I32, _I32, _F, _VP, _I32, _I32, _VP]),
     "sfb_small_linear": (C.c_int, [C.POINTER(SmallLinearParams), _VP]),
     "sfb_im2col_in": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _VP]),
+    "sfb_im2col_in_wide": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _VP]),
     "sfb_conv_in": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "sfb_conv_out": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "sfb_conv_out_temporal": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32,

@@ -192,9 +192,12 @@ class PackedWeights:
         return self._mat(wp)
 
     def conv_in_matrix(self, name):
-        """First conv as a GEMM operand: [cout, (kh, kw, cin)] zero-padded along K to 64."""
-        return self._get(("cin_mat", name), lambda: self._padded_mat(
-            ops.pack_conv3x3(self._raw(name).to(self.device), self.dtype), 64))
+        """First conv as a GEMM operand: [cout, (kh, kw, cin)] zero-padded along K to the next multiple of 64
+        (64 for cin <= 7, 128 for 9 <= cin <= 14)."""
+        def build():
+            w = ops.pack_conv3x3(self._raw(name).to(self.device), self.dtype)
+            return self._padded_mat(w, _round_up(w.shape[1], 64))
+        return self._get(("cin_mat", name), build)
 
     def patch_matrix(self, name, kpad):
         """Patch-embedding conv [cout, cin, p, p] as a GEMM operand over patchified rows: [cout, (cin, p, p)]
@@ -736,6 +739,8 @@ class UNetPlan(Plan):
         self.t_in = self._alloc((batch,), torch.float32)
         self.ehs_in = self._alloc((batch, ctx_len, spec.cross_attention_dim), self.dt)
         self.out = self._alloc((batch, spec.out_channels, height, width), self.dt)
+        if spec.time_cond_dim:  # LCM: the guidance embedding timestep_cond
+            self.timestep_cond_in = self._alloc((batch, spec.time_cond_dim), self.dt)
         if spec.addition_embed_type == "text_time":
             self.add_in = self._alloc((batch, spec.add_in_dim), self.dt)
             self.time_ids_in = self._alloc((batch * 6,), torch.float32)
@@ -1002,6 +1007,13 @@ class UNetPlan(Plan):
                        int(spec.flip_sin_to_cos), float(spec.freq_shift),
                        _ptr(t_emb), c0, ops.dtype_code(self.dt)),
                       (self.t_in, t_emb)))
+        if spec.time_cond_dim:
+            # LCM: diffusers' t_emb + cond_proj(timestep_cond), one fp32 sum rounded once
+            t_cond = self.buf("t_emb_cond", (B, c0))
+            self._emit(ops.small_linear_op("time_embedding.cond_proj", lib, x=self.timestep_cond_in,
+                                           w=self.w.small("time_embedding.cond_proj.weight"), bias=None, batch=B,
+                                           n=c0, k=spec.time_cond_dim, dt=self.dt, y16=t_cond, add16=t_emb))
+            t_emb = t_cond
         h = self.buf("temb_h", (B, spec.temb_dim))
         self._emit(ops.small_linear_op("time_embedding.linear_1", lib, x=t_emb,
                                        w=self.w.small("time_embedding.linear_1.weight"),
@@ -1059,6 +1071,15 @@ class UNetPlan(Plan):
                           (_ptr(self.sample_in), _ptr(a_col), B, H, W, spec.in_channels),
                           (self.sample_in, a_col), 0, B * H * W * 128))
             self.linear("conv_in", Act(a_col, B, H, W, 64), self.w.conv_in_matrix("conv_in.weight"),
+                        self.w.f32("conv_in.bias"), x)
+            self.ops[-1].flops = 2 * B * H * W * x.c * 9 * spec.in_channels  # algorithmic, not padded
+        elif spec.in_channels >= 9:
+            # inpainting (9 channels): K = 9*cin padded to two 64-wide K blocks, the same GEMM
+            a_col = self.buf("conv_in_im2col", (B * H * W, 128))
+            self._emit(Op("conv_in.im2col", lib.sfb_im2col_in_wide,
+                          (_ptr(self.sample_in), _ptr(a_col), B, H, W, spec.in_channels),
+                          (self.sample_in, a_col), 0, B * H * W * (2 * spec.in_channels + 256)))
+            self.linear("conv_in", Act(a_col, B, H, W, 128), self.w.conv_in_matrix("conv_in.weight"),
                         self.w.f32("conv_in.bias"), x)
             self.ops[-1].flops = 2 * B * H * W * x.c * 9 * spec.in_channels  # algorithmic, not padded
         else:

@@ -41,7 +41,7 @@ except Exception:  # noqa: BLE001
             return tuple(self.values())
 
 
-_UNSUPPORTED_KWARGS = ("class_labels", "timestep_cond", "attention_mask", "encoder_attention_mask")
+_UNSUPPORTED_KWARGS = ("class_labels", "attention_mask", "encoder_attention_mask")
 
 
 class LegacyResidualShapeError(ValueError, NotImplementedError):
@@ -339,6 +339,24 @@ class CompiledUNet(_CompiledModule):
                 vals[2 * i], vals[2 * i + 1] = float(getattr(blocks[i], b)), float(getattr(blocks[i], s))
         return on, vals
 
+    def _timestep_cond_input(self, timestep_cond, B):
+        """The [B, time_cond_proj_dim] guidance embedding this call copies into the plan's `timestep_cond_in`, or
+        None for a UNet without time_embedding.cond_proj (which refuses the argument by name).  [1, dim] is
+        broadcast over the batch, as diffusers' add broadcasts it; None is zeros: diffusers then skips the add, and
+        adding an exact zero to the timestep embedding gives the same bits."""
+        dim = self.spec.time_cond_dim
+        if not dim:
+            if timestep_cond is not None:
+                raise NotImplementedError("sfast (H100 build): UNet argument `timestep_cond` is not supported (the "
+                                          "UNet has no time_cond_proj_dim)")
+            return None
+        if timestep_cond is None:
+            return torch.zeros(B, dim)
+        shape = tuple(timestep_cond.shape)
+        if shape not in ((B, dim), (1, dim)):
+            raise ValueError(f"timestep_cond of shape {shape}: expected [{B}, {dim}] or [1, {dim}]")
+        return timestep_cond.expand(B, dim)
+
     # -- forward -------------------------------------------------------------------------
     def _call_svd(self, sample, timestep, encoder_hidden_states, added_time_ids, return_dict=True):
         """diffusers UNetSpatioTemporalConditionModel.forward(sample [B, F, C, H, W], timestep,
@@ -384,12 +402,13 @@ class CompiledUNet(_CompiledModule):
                  added_cond_kwargs=None, down_block_additional_residuals=None,
                  mid_block_additional_residual=None, down_intrablock_additional_residuals=None,
                  encoder_attention_mask=None, return_dict=True):
-        given = dict(class_labels=class_labels, timestep_cond=timestep_cond,
-                     attention_mask=attention_mask, encoder_attention_mask=encoder_attention_mask)
+        given = dict(class_labels=class_labels, attention_mask=attention_mask,
+                     encoder_attention_mask=encoder_attention_mask)
         for k in _UNSUPPORTED_KWARGS:
             if given[k] is not None:
                 raise NotImplementedError(f"sfast (H100 build): UNet argument `{k}` is not supported")
         B, _, H, W = sample.shape
+        t_cond = self._timestep_cond_input(timestep_cond, B)
         ip_len, ip_seq, image_embeds, ip_scales = self._ip_inputs(added_cond_kwargs, cross_attention_kwargs, B)
         lora_scale = 1.0
         if cross_attention_kwargs:
@@ -435,6 +454,8 @@ class CompiledUNet(_CompiledModule):
             t = timestep if torch.is_tensor(timestep) else torch.tensor(float(timestep))
             t = t.reshape(-1).to(device=sample.device, dtype=torch.float32, non_blocking=True)
             plan.t_in.copy_(t.expand(B) if t.numel() == 1 else t)
+            if t_cond is not None:
+                plan.timestep_cond_in.copy_(t_cond)
             if self.spec.addition_embed_type == "text_time":
                 if not added_cond_kwargs or "text_embeds" not in added_cond_kwargs:
                     raise ValueError("added_cond_kwargs with text_embeds / time_ids is required")

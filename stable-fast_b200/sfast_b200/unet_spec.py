@@ -125,6 +125,9 @@ class UNetSpec:
     cond_embed_channels: tuple = ()
     cond_bgr: bool = False
     ip: Optional[IPAdapterSpec] = None  # an IP-Adapter is loaded (UNet only)
+    # LCM (diffusers time_cond_proj_dim, UNet only): width of the guidance embedding `timestep_cond` that
+    # time_embedding.cond_proj (no bias) projects and adds to the sinusoidal timestep embedding; 0: none
+    time_cond_dim: int = 0
 
     @property
     def temporal(self):
@@ -164,7 +167,8 @@ def spec_from_config(cfg) -> UNetSpec:
         return svd_spec_from_config(cfg)
     # an IP-Adapter sets encoder_hid_dim_type = "ip_image_proj"; its geometry is read from the module
     # (ip_adapter_spec), not the config.  A ControlNet never receives image embeddings: it keeps refusing it.
-    spec, tf, layers = _encoder_spec(cfg, out_channels=cfg_get(cfg, "out_channels", 4), accept_ip=True)
+    spec, tf, layers = _encoder_spec(cfg, out_channels=cfg_get(cfg, "out_channels", 4), accept_ip=True,
+                                     accept_time_cond=True)
     up_types = tuple(cfg_get(cfg, "up_block_types"))
     for t in up_types:
         if t not in _SUPPORTED_UP:
@@ -189,22 +193,27 @@ def spec_from_config(cfg) -> UNetSpec:
     return spec
 
 
-def _encoder_spec(cfg, out_channels, accept_ip=False):
+def _encoder_spec(cfg, out_channels, accept_ip=False, accept_time_cond=False):
     """The part of the architecture a UNet and a ControlNet share (time embedding, conv_in, down blocks,
     mid block), with every check of the config keys both carry.  Returns (spec without up blocks, the
     transformer-spec factory, layers per block).  `accept_ip`: encoder_hid_dim_type="ip_image_proj" (an
-    IP-Adapter) passes; the caller reads the adapter from the module."""
+    IP-Adapter) passes; the caller reads the adapter from the module.  `accept_time_cond`: time_cond_proj_dim
+    (an LCM's guidance embedding) passes."""
     boc = tuple(cfg_get(cfg, "block_out_channels"))
     nb = len(boc)
     down_types = tuple(cfg_get(cfg, "down_block_types"))
     for t in down_types:
         if t not in _SUPPORTED_DOWN:
             raise NotImplementedError(f"down block type {t} is not supported by the H100 path")
+    # upcast_attention (SD-2.1 768-v) only makes diffusers' legacy AttnProcessor compute QK^T in fp32; the fused
+    # attention always accumulates QK^T and runs the softmax in fp32, so both values compute the same
     for key in ("class_embed_type", "encoder_hid_dim_type", "time_cond_proj_dim",
                 "resnet_time_scale_shift", "dual_cross_attention", "only_cross_attention",
-                "upcast_attention", "time_embedding_act_fn", "attention_type"):
+                "time_embedding_act_fn", "attention_type"):
         v = cfg_get(cfg, key)
         if accept_ip and key == "encoder_hid_dim_type" and v == "ip_image_proj":
+            continue
+        if accept_time_cond and key == "time_cond_proj_dim" and v is not None:
             continue
         if v not in (None, False, "default", "positional"):
             raise NotImplementedError(f"UNet config {key}={v!r} is not supported by the H100 path")
@@ -219,7 +228,7 @@ def _encoder_spec(cfg, out_channels, accept_ip=False):
         "addition_embed_type_num_heads": (64,), "timestep_post_act": (None,),
         "time_embedding_dim": (None,), "class_embeddings_concat": (False,),
         "reverse_transformer_layers_per_block": (None,), "dropout": (0, 0.0),
-        "center_input_sample": (False,), "encoder_hid_dim": (None,),
+        "center_input_sample": (False,), "encoder_hid_dim": (None,), "upcast_attention": (None, False, True),
     }
     for key, allowed in required.items():
         v = cfg_get(cfg, key, allowed[0])
@@ -247,14 +256,24 @@ def _encoder_spec(cfg, out_channels, accept_ip=False):
     add_type = cfg_get(cfg, "addition_embed_type")
     if add_type not in (None, "text_time"):
         raise NotImplementedError(f"addition_embed_type={add_type}")
+    cin = cfg_get(cfg, "in_channels", 4)
+    if cin > 14:
+        # conv_in's im2col rows hold 9 * in_channels columns in at most two 64-wide K blocks
+        raise NotImplementedError(f"UNet config in_channels={cin} is not supported by the H100 path "
+                                  "(supported: 1 to 14)")
+    time_cond = cfg_get(cfg, "time_cond_proj_dim") if accept_time_cond else None
+    if time_cond is not None and (int(time_cond) <= 0 or int(time_cond) % 8):
+        # cond_proj runs on sfb_small_linear, whose K is read in 8-element vectors
+        raise NotImplementedError(f"UNet config time_cond_proj_dim={time_cond!r} is not supported by the H100 "
+                                  "path (supported: a positive multiple of 8)")
     spec = UNetSpec(
-        in_channels=cfg_get(cfg, "in_channels", 4), out_channels=out_channels,
+        in_channels=cin, out_channels=out_channels,
         block_out_channels=boc, temb_dim=boc[0] * 4, groups=cfg_get(cfg, "norm_num_groups", 32),
         eps=cfg_get(cfg, "norm_eps", 1e-5), flip_sin_to_cos=cfg_get(cfg, "flip_sin_to_cos", True),
         freq_shift=float(cfg_get(cfg, "freq_shift", 0)), cross_attention_dim=ctx,
         addition_embed_type=add_type,
         addition_time_embed_dim=cfg_get(cfg, "addition_time_embed_dim"),
-        add_in_dim=cfg_get(cfg, "projection_class_embeddings_input_dim"))
+        add_in_dim=cfg_get(cfg, "projection_class_embeddings_input_dim"), time_cond_dim=int(time_cond or 0))
 
     def tf(prefix, dim, i):
         return TransformerSpec(prefix, dim, heads[i], depth[i], ctx, linear)
@@ -645,6 +664,8 @@ def param_shapes(spec: UNetSpec):
 
     conv("conv_in", spec.block_out_channels[0], spec.in_channels, 3)
     lin("time_embedding.linear_1", spec.temb_dim, spec.block_out_channels[0])
+    if spec.time_cond_dim:  # diffusers' TimestepEmbedding(cond_proj_dim=...): no bias
+        lin("time_embedding.cond_proj", spec.block_out_channels[0], spec.time_cond_dim, False)
     lin("time_embedding.linear_2", spec.temb_dim, spec.temb_dim)
     if spec.addition_embed_type in ("text_time", "time_ids"):
         lin("add_embedding.linear_1", spec.temb_dim, spec.add_in_dim)

@@ -402,6 +402,30 @@ typedef struct sfb_temporal_attn_params {
 
 int sfb_temporal_attention(const sfb_temporal_attn_params* p, sfb_stream_t stream);
 
+/* ---- AnimateDiff motion modules (diffusers UNetMotionModel; the reference traces the module) ---------- */
+
+/* Self-attention across frames on the tensor cores: for every (video b, pixel p, head h) a sequence of `frames`
+ * tokens, softmax(scale * q k^T) v with fp32 accumulation and an fp32 softmax.
+ *   qkv:        [batch * frames * seq, ld_qkv] 16-bit = q | k | v column blocks of heads * head_dim each, in the
+ *               SPATIAL row order m = (b * frames + f) * seq + p; out [same rows, ld_out] receives heads * head_dim
+ *               columns in the same order;
+ *   frame_bias: fp32 [frames, ld_bias] (q | k | v columns like qkv) or NULL: row f is added to the q / k / v of
+ *               frame f as they are loaded (the sum is rounded to 16 bits once) -- a position embedding added
+ *               in front of the projections, (x + pe_f) W^T = x W^T + pe_f W^T.
+ * 1 <= frames <= 32, head_dim 40, 80 or 160, scale > 0; ld_qkv >= 3 * heads * head_dim and ld_out >= heads *
+ * head_dim are multiples of 8; ld_bias >= 3 * heads * head_dim is a multiple of 4; pointers are 16-byte
+ * aligned; out must not overlap qkv. */
+typedef struct sfb_frame_attn_params {
+    const void* qkv;
+    const float* frame_bias;
+    void* out;
+    int32_t batch, frames, seq, heads, head_dim;
+    int32_t ld_qkv, ld_bias, ld_out, dtype;
+    float scale;
+} sfb_frame_attn_params;
+
+int sfb_frame_attention(const sfb_frame_attn_params* p, sfb_stream_t stream);
+
 enum sfb_row_index_mode {
     SFB_ROW_IDX_DIV_MOD = 0,      /* vec row = (m / div) % mod */
     SFB_ROW_IDX_TEMPORAL_CTX = 1, /* vec row = ((b * seq + p) % batch) * frames, m = (b*frames + f)*seq + p:

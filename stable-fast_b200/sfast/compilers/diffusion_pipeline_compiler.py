@@ -58,7 +58,9 @@ def compile(m, config):
     residuals (``down_intrablock_additional_residuals``) inside its step.  A loaded IP-Adapter (one plain ``ImageProjection`` or one
     IP-Adapter Plus ``IPAdapterPlusImageProjection``) runs inside the UNet's step, see `compile_unet`.  PEFT LoRA
     adapters on the UNet and the text encoders are merged into their packed weights (see `compile_unet`); adapters
-    on the ControlNet, the VAE or the vision tower raise ``NotImplementedError`` at their first call."""
+    on the ControlNet, the VAE or the vision tower raise ``NotImplementedError`` at their first call.  An AnimateDiff
+    pipeline's ``UNetMotionModel`` runs natively with its motion modules (see `compile_unet`); a
+    ``SparseControlNetModel`` stays eager and its residuals reach the native UNet like any ControlNet's."""
     m.unet = compile_unet(m.unet, config)
     if getattr(m, 'controlnet', None) is not None:
         m.controlnet = compile_controlnet(m.controlnet, config)
@@ -197,7 +199,16 @@ def compile_unet(m, config):
     ``[1]`` on every call, with diffusers' rule per block (on when all four of its values are truthy): the
     backbone scaling and the Fourier skip filter run natively in front of each resnet of those blocks, inside the
     CUDA graph.  Each on/off pair gets its own plan; changing the values reuses it, and with FreeU off the step
-    is the plain one."""
+    is the plain one.
+
+    AnimateDiff's ``UNetMotionModel`` (``forward(sample [B, C, F, H, W], timestep, encoder_hidden_states, ...)``)
+    runs as B*F images with the motion modules inside the same step: the video GroupNorm, proj_in, the two
+    self-attentions across the frames (with the sinusoidal position embedding) and the GEGLU FeedForward of each
+    block, and proj_out.  One plan and CUDA graph per (B, F, H, W, dtype, ControlNet or not); ``timestep_cond``
+    (AnimateLCM) and SDXL's ``added_cond_kwargs`` are repeated per frame, ControlNet residuals are ``[B*F, C, h,
+    w]``, and PEFT LoRA adapters, motion LoRAs included, are merged as above.  ``attention_mask``, an IP-Adapter,
+    FreeU, T2I-Adapter residuals, FreeNoise and more frames than ``motion_max_seq_length`` raise
+    ``NotImplementedError`` by name on the call that uses them."""
     from sfast_b200.runtime import compile_unet_module, require_sm90
     device = m.device if hasattr(m, 'device') else torch.device(
         'cuda' if torch.cuda.is_available() else 'cpu')

@@ -102,6 +102,13 @@ class TemporalAttnParams(C.Structure):
                 ("scale", C.c_float)]
 
 
+class FrameAttnParams(C.Structure):
+    _fields_ = [("qkv", C.c_void_p), ("frame_bias", C.c_void_p), ("out", C.c_void_p),
+                ("batch", C.c_int32), ("frames", C.c_int32), ("seq", C.c_int32), ("heads", C.c_int32),
+                ("head_dim", C.c_int32), ("ld_qkv", C.c_int32), ("ld_bias", C.c_int32), ("ld_out", C.c_int32),
+                ("dtype", C.c_int32), ("scale", C.c_float)]
+
+
 class RowOpParams(C.Structure):
     _fields_ = [("x", C.c_void_p), ("x2", C.c_void_p), ("vec", C.c_void_p), ("y", C.c_void_p),
                 ("rowstats_out", C.c_void_p), ("mix_factor", C.c_void_p),
@@ -193,6 +200,7 @@ SYMBOLS = {
                                         _I32, _VP]),
     "sfb_upsample2x": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "sfb_temporal_attention": (C.c_int, [C.POINTER(TemporalAttnParams), _VP]),
+    "sfb_frame_attention": (C.c_int, [C.POINTER(FrameAttnParams), _VP]),
     "sfb_row_broadcast_add": (C.c_int, [C.POINTER(RowOpParams), _VP]),
     "sfb_alpha_blend": (C.c_int, [C.POINTER(RowOpParams), _VP]),
     "sfb_add_nchw_residuals": (C.c_int, [C.POINTER(AddNchwParams), _VP]),

@@ -262,6 +262,18 @@ class PackedWeights:
             return (self._mat(wt), bp, inner, cs)
         return self._get(("lngeglu", prefix, ln_prefix), build)
 
+    def frame_bias_table(self, names, pe_name, max_seq):
+        """fp32 pe[0, :max_seq] cat(names)^T -> [max_seq, sum of the rows of names]: a position embedding added
+        after a LayerNorm's affine and in front of the projections `names` (AnimateDiff's motion attentions), as
+        the per-frame bias sfb_frame_attention adds to q | k | v.  The LayerNorm stays folded into the QKV GEMM,
+        which cannot also take a row bias: (LN(x) + pe_f) W^T = LN(x) W^T + pe_f W^T.  Built from the same
+        state-dict names as the QKV matrix, so a parameter update or a LoRA merge re-packs both."""
+        def build():
+            w = torch.cat([self._raw(n).to(self.device).float() for n in names], 0)
+            pe = self._raw(pe_name).to(self.device).float()[0, :max_seq]
+            return (pe @ w.t()).contiguous()
+        return self._get(("frame_bias", pe_name, max_seq) + tuple(names), build)
+
     def geglu(self, prefix):
         def build():
             wp, bp, inner = ops.pack_geglu(self._raw(prefix + ".weight").to(self.device),
@@ -668,8 +680,8 @@ class Plan:
 
 class VideoPlanMixin:
     """Emitters of a plan whose batch is `nvid` videos of `F` consecutive frames (both set by the plan) --
-    the SVD UNet and SVD's temporal VAE decoder.  Frames are a batch of images for everything spatial; a
-    temporal operator works on the same token-major [B*F*H*W, C] tensors viewed as [B, F, H*W, C]."""
+    the SVD UNet, SVD's temporal VAE decoder and the AnimateDiff UNet.  Frames are a batch of images for everything
+    spatial; a temporal operator works on the same token-major [B*F*H*W, C] tensors viewed as [B, F, H*W, C]."""
 
     def _video_view(self, x: Act):
         """[B*F, h, w, c] -> [B, F*h, w, c]: GroupNorm statistics over (frames, height, width)."""
@@ -677,6 +689,17 @@ class VideoPlanMixin:
 
     def _frame_view(self, y: Act, like: Act):
         return Act(y.buf, like.n, like.h, like.w, y.c, ld=y.ld, off=y.off)
+
+    def _ff(self, b, ffname, ln_prefix, hs: Act, st, stats_next, dim):
+        """hs += ff(LayerNorm(hs)): GEGLU projection (LayerNorm folded) + output projection."""
+        gm, bp, inner, colsum = self.w.ln_geglu(f"{b}.{ffname}.net.0.proj", ln_prefix)
+        ff = self.act("ff_act", hs.n, hs.h, hs.w, inner)
+        self._emit(self._gemm(f"{b}.{ffname}.geglu", a=self._a_matrix(hs), b=gm, M=hs.rows, N=gm.n, K=dim,
+                              dt=self.dt, out=ff.ptr, ldo=inner, bias=bp, epi=EPI_GEGLU, geglu_n_out=inner,
+                              ln=dict(rowstats=st, colsum=colsum, eps=1e-5, dim=dim),
+                              keep=(hs.buf, ff.buf, gm, colsum)))
+        self.linear(f"{b}.{ffname}.out", ff, self.w.matrix(f"{b}.{ffname}.net.2.weight"),
+                    self.w.f32(f"{b}.{ffname}.net.2.bias"), hs, residual=hs, rowstats_out=stats_next)
 
     def conv3x1_t(self, name, x: Act, wm, bias, dst: Act, rowbias=None, residual: Act = None):
         """Conv3d (3,1,1), padding (1,0,0) over the frame axis of x viewed as [B, F, H*W, C]."""
@@ -698,6 +721,8 @@ class VideoPlanMixin:
 class UNetPlan(Plan):
     """One static launch schedule of the UNet for a fixed (batch, height, width)."""
 
+    _motion = False  # MotionUNetPlan: emits the motion modules of spec.motion
+
     def __init__(self, weights: PackedWeights, batch, height, width, ctx_len=77, controlnet=False, ip_len=0,
                  ip_seq=0, intrablock=0, freeu=(False, False)):
         """`ip_len` > 0: an IP-Adapter (spec.ip) adds ip_len image tokens per sample (n_img images x its
@@ -709,6 +734,8 @@ class UNetPlan(Plan):
         its resnets with the values of the static input `freeu_in` = (b1, s1, b2, s2); (False, False) builds
         exactly the schedule without it."""
         spec = weights.spec
+        if spec.motion and not self._motion:
+            raise ValueError("a UNetMotionModel spec (spec.motion) is built by motion_plan.MotionUNetPlan")
         div = 1 << (len(spec.block_out_channels) - 1)
         if height % div or width % div:
             # diffusers switches to explicit upsample sizes there (forward_upsample_size); not built
@@ -716,7 +743,7 @@ class UNetPlan(Plan):
                 f"sfast (H100 build): latent size {height}x{width} must be a multiple of {div}")
         # (+1: conv_norm_out, the head of the up path; a ControlNet has none)
         n_gn = sum(2 for _ in spec.all_resnets()) + (1 if spec.up else 0) + sum(
-            1 for blk in spec.down + [spec.mid] + spec.up for t in blk.attentions if t is not None)
+            1 for blk in spec.down + [spec.mid] + spec.up for t in blk.attentions if t is not None) + len(spec.motion)
         super().__init__(weights, batch, height, width, n_gn=n_gn,
                          ln_floats=self._ln_arena_floats(spec, batch, height, width))
         self.ctx_len = ctx_len

@@ -16,6 +16,7 @@ import time
 import torch
 
 from . import lora
+from .motion_plan import MotionUNetPlan
 from .plan import PackedWeights, UNetPlan, intrablock_shapes
 from .svd_plan import SVDPlan
 from .unet_spec import cfg_get, ip_adapter_spec, ip_scale_of, spec_from_config
@@ -39,6 +40,12 @@ except Exception:  # noqa: BLE001
 
         def to_tuple(self):
             return tuple(self.values())
+
+
+try:  # the AnimateDiff UNet's output class (diffusers >= 0.28); the 2-D one has the same fields
+    from diffusers.models.unets.unet_motion_model import UNetMotionOutput  # type: ignore
+except Exception:  # noqa: BLE001
+    UNetMotionOutput = UNet2DConditionOutput
 
 
 _UNSUPPORTED_KWARGS = ("class_labels", "attention_mask", "encoder_attention_mask")
@@ -246,7 +253,9 @@ class CompiledUNet(_CompiledModule):
         self._module = module
         self._ip_proj = getattr(module, "encoder_hid_proj", None)
         self._ip_procs = None
-        if cfg_get(config, "encoder_hid_dim_type") == "ip_image_proj" or self._ip_proj is not None:
+        if spec.motion:
+            pass  # an IP-Adapter on the motion UNet is refused by name on every call (_motion_refusals)
+        elif cfg_get(config, "encoder_hid_dim_type") == "ip_image_proj" or self._ip_proj is not None:
             if module is None:
                 raise NotImplementedError("sfast (H100 build): an IP-Adapter UNet is compiled from the module "
                                           "(compile_unet_module), not from its config alone")
@@ -392,9 +401,109 @@ class CompiledUNet(_CompiledModule):
             return (out,)
         return UNet2DConditionOutput(sample=out)
 
+    def _motion_refusals(self, attention_mask, down_intrablock_additional_residuals):
+        """NotImplementedError naming what the motion UNet's plan does not compute.  Everything here can change
+        after compile() (an adapter loaded, FreeU or FreeNoise switched on), so it is checked on every call."""
+        def refuse(what):
+            raise NotImplementedError(f"sfast (H100 build): {what} is not supported by the H100 path on the "
+                                      "AnimateDiff UNet (UNetMotionModel)")
+        if attention_mask is not None:
+            refuse("UNet argument `attention_mask`")
+        if down_intrablock_additional_residuals is not None:
+            refuse("`down_intrablock_additional_residuals` (T2I-Adapter)")
+        m = self._module
+        if cfg_get(getattr(m, "config", None), "encoder_hid_dim_type") == "ip_image_proj" or \
+                getattr(m, "encoder_hid_proj", None) is not None:
+            refuse("an IP-Adapter")
+        if m is None:
+            return
+        if any(getattr(blk, k, None) for blk in getattr(m, "up_blocks", ()) for k in ("s1", "s2", "b1", "b2")):
+            refuse("FreeU (enable_freeu)")
+        for mm in self.spec.motion:
+            try:
+                mod = m.get_submodule(mm.prefix)
+            except AttributeError:
+                continue
+            for blk in getattr(mod, "transformer_blocks", ()):
+                if type(blk).__name__ == "FreeNoiseTransformerBlock":
+                    refuse(f"FreeNoise (enable_free_noise: {mm.prefix} runs FreeNoiseTransformerBlock)")
+
+    def _call_motion(self, sample, timestep, encoder_hidden_states, timestep_cond=None, attention_mask=None,
+                     cross_attention_kwargs=None, added_cond_kwargs=None, down_block_additional_residuals=None,
+                     mid_block_additional_residual=None, down_intrablock_additional_residuals=None, return_dict=True):
+        """diffusers UNetMotionModel.forward(sample [B, C, F, H, W], timestep, encoder_hidden_states [B, L, ctx],
+        ...): the F frames of each video are a batch of B*F images, and the time embedding (with an LCM's
+        timestep_cond and SDXL's added_cond_kwargs) and the prompt are repeated per frame, as diffusers repeats
+        them.  ControlNet residuals are [B*F, C, h, w].  Returns [B, C_out, F, H, W]."""
+        self._motion_refusals(attention_mask, down_intrablock_additional_residuals)
+        if sample.dim() != 5:
+            raise ValueError(f"sample of shape {tuple(sample.shape)}: the motion UNet takes [B, C, F, H, W]")
+        B, _, F_, H, W = sample.shape
+        max_seq = min(m.max_seq_len for m in self.spec.motion)
+        if F_ > max_seq:
+            raise NotImplementedError(f"sfast (H100 build): {F_} frames; the motion modules take at most "
+                                      f"motion_max_seq_length = {max_seq} (FreeNoise's sliding windows are not "
+                                      "supported)")
+        t_cond = self._timestep_cond_input(timestep_cond, B)
+        lora_scale = 1.0
+        if cross_attention_kwargs:
+            lora_scale = float(cross_attention_kwargs.get("scale", 1.0))
+            if set(cross_attention_kwargs) - {"scale"} or (lora_scale != 1.0 and (self._lora is None or self._lora.quiet())):
+                raise NotImplementedError("sfast (H100 build): cross_attention_kwargs (LoRA scale) "
+                                          "is not supported; fuse the LoRA weights into the parameters")
+        require_sm90(sample.device)
+        dtype = sample.dtype
+        if dtype not in (torch.float16, torch.bfloat16):
+            raise NotImplementedError(f"sfast (H100 build): UNet dtype {dtype}; use fp16 or bf16")
+        controlnet = down_block_additional_residuals is not None or mid_block_additional_residual is not None
+        if controlnet and (down_block_additional_residuals is None or mid_block_additional_residual is None):
+            raise NotImplementedError("sfast (H100 build): ControlNet residuals need both "
+                                      "down_block_additional_residuals and mid_block_additional_residual")
+        ctx_len = encoder_hidden_states.shape[1]
+        with self._lock, torch.cuda.device(sample.device):
+            t_first = time.perf_counter() if self.first_call_s is None else None
+            weights = self._weights_for(dtype, sample.device, lora_scale)
+            gp = self._graphed(("motion", B, F_, H, W, dtype, ctx_len, sample.device.index, controlnet),
+                               lambda: MotionUNetPlan(weights, B, F_, H, W, ctx_len, controlnet=controlnet))
+            plan = gp.plan
+            # [B, C, F, H, W] -> the static [B*F, C, H, W] input, permuted by the copy itself
+            plan.sample_in.view(B, F_, -1, H, W).copy_(sample.permute(0, 2, 1, 3, 4), non_blocking=True)
+            plan.ehs_in.view(B, F_, ctx_len, -1).copy_(encoder_hidden_states.unsqueeze(1), non_blocking=True)
+            t = timestep if torch.is_tensor(timestep) else torch.tensor(float(timestep))
+            t = t.reshape(-1).to(device=sample.device, dtype=torch.float32, non_blocking=True)
+            plan.t_in.copy_((t.expand(B) if t.numel() == 1 else t).repeat_interleave(F_))
+            if t_cond is not None:
+                plan.timestep_cond_in.copy_(t_cond.repeat_interleave(F_, dim=0))
+            if self.spec.addition_embed_type == "text_time":
+                if not added_cond_kwargs or "text_embeds" not in added_cond_kwargs:
+                    raise ValueError("added_cond_kwargs with text_embeds / time_ids is required")
+                te = added_cond_kwargs["text_embeds"]
+                plan.add_in[:, :te.shape[1]].copy_(te.repeat_interleave(F_, dim=0))
+                plan.time_ids_in.copy_(added_cond_kwargs["time_ids"].reshape(B, -1).float()
+                                       .repeat_interleave(F_, dim=0).reshape(-1))
+            if controlnet:
+                res = list(down_block_additional_residuals) + [mid_block_additional_residual]
+                if len(res) != len(plan.ctrl_in):
+                    raise ValueError(f"expected {len(plan.ctrl_in) - 1} down-block residuals, got {len(res) - 1}")
+                for dst, src in zip(plan.ctrl_in, res):
+                    if tuple(src.shape) != tuple(dst.shape):
+                        raise ValueError(f"ControlNet residual shape {tuple(src.shape)} != {tuple(dst.shape)} "
+                                         "(the motion UNet takes [B * frames, C, h, w])")
+                    dst.copy_(src, non_blocking=True)
+            gp.step()
+            out = plan.out.view(B, F_, -1, H, W).permute(0, 2, 1, 3, 4).contiguous()
+            if t_first is not None:
+                torch.cuda.current_stream().synchronize()
+                self.first_call_s = time.perf_counter() - t_first
+        if not return_dict:
+            return (out,)
+        return UNetMotionOutput(sample=out)
+
     def __call__(self, sample, timestep, encoder_hidden_states, *args, **kwargs):
         if self.spec.temporal:
             return self._call_svd(sample, timestep, encoder_hidden_states, *args, **kwargs)
+        if self.spec.motion:
+            return self._call_motion(sample, timestep, encoder_hidden_states, *args, **kwargs)
         return self._call_2d(sample, timestep, encoder_hidden_states, *args, **kwargs)
 
     def _call_2d(self, sample, timestep, encoder_hidden_states, class_labels=None,

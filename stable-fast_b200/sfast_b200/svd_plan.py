@@ -24,7 +24,7 @@ import ctypes as C
 import torch
 
 from . import _lib, ops
-from .ops import Act, EPI_GEGLU, Op, _ptr
+from .ops import Act, Op, _ptr
 from .plan import UNetPlan, VideoPlanMixin, _JoinOp
 
 
@@ -175,17 +175,6 @@ class SVDPlan(VideoPlanMixin, UNetPlan):
         if not self._joined:
             self._joined = True
             self._emit(_JoinOp("all"))
-
-    def _ff(self, b, ffname, ln_prefix, hs: Act, st, stats_next, dim):
-        """hs += ff(LayerNorm(hs)): GEGLU projection (LayerNorm folded) + output projection."""
-        gm, bp, inner, colsum = self.w.ln_geglu(f"{b}.{ffname}.net.0.proj", ln_prefix)
-        ff = self.act("ff_act", hs.n, hs.h, hs.w, inner)
-        self._emit(self._gemm(f"{b}.{ffname}.geglu", a=self._a_matrix(hs), b=gm, M=hs.rows, N=gm.n, K=dim,
-                              dt=self.dt, out=ff.ptr, ldo=inner, bias=bp, epi=EPI_GEGLU, geglu_n_out=inner,
-                              ln=dict(rowstats=st, colsum=colsum, eps=1e-5, dim=dim),
-                              keep=(hs.buf, ff.buf, gm, colsum)))
-        self.linear(f"{b}.{ffname}.out", ff, self.w.matrix(f"{b}.{ffname}.net.2.weight"),
-                    self.w.f32(f"{b}.{ffname}.net.2.bias"), hs, residual=hs, rowstats_out=stats_next)
 
     def transformer(self, t, x: Act, dst: Act):
         if not t.temporal:

@@ -102,6 +102,31 @@ class IPAdapterSpec:
 
 
 @dataclass
+class MotionSpec:
+    """One AnimateDiff motion module (diffusers ``AnimateDiffTransformer3D``, formerly
+    ``TransformerTemporalModel``) at `prefix`: a video GroupNorm of `groups` groups, proj_in, `depth`
+    BasicTransformerBlocks whose two self-attentions run across the frames with the sinusoidal position
+    embedding of `max_seq_len` positions, proj_out, and the residual.  `after`: the module that produces its
+    input (the layer's resnet or transformer prefix)."""
+    prefix: str
+    dim: int
+    heads: int
+    depth: int
+    max_seq_len: int
+    groups: int
+    after: str = ""
+
+    @property
+    def head_dim(self):
+        return self.dim // self.heads
+
+
+# head sizes sfb_frame_attention compiles
+MOTION_HEAD_DIMS = (40, 80, 160)
+MOTION_MAX_FRAMES = 32
+
+
+@dataclass
 class UNetSpec:
     in_channels: int
     out_channels: int
@@ -128,6 +153,8 @@ class UNetSpec:
     # LCM (diffusers time_cond_proj_dim, UNet only): width of the guidance embedding `timestep_cond` that
     # time_embedding.cond_proj (no bias) projects and adds to the sinusoidal timestep embedding; 0: none
     time_cond_dim: int = 0
+    # AnimateDiff (diffusers UNetMotionModel): the motion modules in schedule order; [] for every other UNet
+    motion: List[MotionSpec] = field(default_factory=list)
 
     @property
     def temporal(self):
@@ -165,6 +192,8 @@ _SUPPORTED_UP = ("CrossAttnUpBlock2D", "UpBlock2D")
 def spec_from_config(cfg) -> UNetSpec:
     if is_svd_config(cfg):
         return svd_spec_from_config(cfg)
+    if is_motion_config(cfg):
+        return motion_spec_from_config(cfg)
     # an IP-Adapter sets encoder_hid_dim_type = "ip_image_proj"; its geometry is read from the module
     # (ip_adapter_spec), not the config.  A ControlNet never receives image embeddings: it keeps refusing it.
     spec, tf, layers = _encoder_spec(cfg, out_channels=cfg_get(cfg, "out_channels", 4), accept_ip=True,
@@ -494,6 +523,108 @@ def ip_scale_of(proc, prefix):
     return float(s)
 
 
+_MOTION_TYPES = {"CrossAttnDownBlockMotion": "CrossAttnDownBlock2D", "DownBlockMotion": "DownBlock2D",
+                 "CrossAttnUpBlockMotion": "CrossAttnUpBlock2D", "UpBlockMotion": "UpBlock2D"}
+
+
+def is_motion_config(cfg):
+    return any(str(t).endswith("Motion") for t in (cfg_get(cfg, "down_block_types") or ()))
+
+
+class _Config2D:
+    """A UNetMotionModel config read as the 2-D UNet config it extends: the Motion block types become their
+    2-D counterparts, every other key is the config's own."""
+
+    def __init__(self, cfg):
+        self._cfg = cfg
+        self._over = {k: tuple(_MOTION_TYPES.get(t, t) for t in cfg_get(cfg, k))
+                      for k in ("down_block_types", "up_block_types")}
+
+    def __getattr__(self, key):
+        if key.startswith("_"):
+            raise AttributeError(key)
+        if key in self._over:
+            return self._over[key]
+        v = cfg_get(self._cfg, key, _MISSING)
+        if v is _MISSING:
+            raise AttributeError(key)
+        return v
+
+
+_MISSING = object()
+
+
+def motion_spec_from_config(cfg) -> UNetSpec:
+    """diffusers ``UNetMotionModel`` (AnimateDiff): the SD-1.5 / SDXL UNet it extends, built from the same
+    config with the Motion block types read as their 2-D counterparts, plus one MotionSpec per motion module in
+    schedule order -- after every (resnet, transformer) layer of the down and up blocks and, with
+    use_motion_mid_block, between the mid block's transformer and its second resnet.  What the plan would compute
+    differently is refused by name."""
+    def refuse(what, supported):
+        raise NotImplementedError(f"UNetMotionModel config {what} is not supported by the H100 path "
+                                  f"(supported: {supported})")
+    for t in tuple(cfg_get(cfg, "down_block_types")) + tuple(cfg_get(cfg, "up_block_types")):
+        if t not in _MOTION_TYPES:
+            raise NotImplementedError(f"block type {t} is not supported by the H100 path in a UNetMotionModel")
+    spec = spec_from_config(_Config2D(cfg))
+    boc = spec.block_out_channels
+    nb = len(boc)
+    mid_layers = cfg_get(cfg, "mid_block_layers", 1)
+    if mid_layers != 1:
+        refuse(f"mid_block_layers={mid_layers!r}", "1")
+    mid_depth = cfg_get(cfg, "transformer_layers_per_mid_block")
+    if mid_depth is not None:
+        spec.mid.attentions[0].depth = int(mid_depth)
+    heads = _tuple(cfg_get(cfg, "motion_num_attention_heads", 8), nb)
+    depth = _tuple(cfg_get(cfg, "temporal_transformer_layers_per_block", 1), nb)
+    for key, fwd in (("reverse_motion_num_attention_heads", heads),
+                     ("reverse_temporal_transformer_layers_per_block", depth)):
+        v = cfg_get(cfg, key)
+        if v is not None and _tuple(v, nb) != tuple(reversed(fwd)):
+            refuse(f"{key}={v!r}", f"None or the reversed forward values {tuple(reversed(fwd))}")
+    max_seq = int(cfg_get(cfg, "motion_max_seq_length", 32))
+    if not 1 <= max_seq <= MOTION_MAX_FRAMES:
+        refuse(f"motion_max_seq_length={max_seq}", f"1 to {MOTION_MAX_FRAMES}")
+    groups = int(cfg_get(cfg, "motion_norm_num_groups", 32))
+    if groups != spec.groups:
+        refuse(f"motion_norm_num_groups={groups}", f"norm_num_groups = {spec.groups}")
+
+    def motion(prefix, dim, h, d, after):
+        if dim % h or dim // h not in MOTION_HEAD_DIMS:
+            refuse(f"motion head_dim {dim}/{h} at {prefix}", f"one of {MOTION_HEAD_DIMS}")
+        return MotionSpec(prefix, dim, h, int(d), max_seq, groups, after)
+
+    for i, blk in enumerate(spec.down):
+        for j, (r, t) in enumerate(zip(blk.resnets, blk.attentions)):
+            spec.motion.append(motion(f"{blk.prefix}.motion_modules.{j}", blk.cout, heads[i], depth[i],
+                                      (t or r).prefix))
+    if cfg_get(cfg, "use_motion_mid_block", True):
+        mdepth = cfg_get(cfg, "temporal_transformer_layers_per_mid_block", 1)
+        if isinstance(mdepth, (list, tuple)):
+            if len(mdepth) != 1:
+                refuse(f"temporal_transformer_layers_per_mid_block={mdepth!r}", "one value (mid_block_layers = 1)")
+            mdepth = mdepth[0]
+        spec.motion.append(motion("mid_block.motion_modules.0", boc[-1], heads[-1], mdepth,
+                                  spec.mid.attentions[0].prefix))
+    rheads, rdepth = tuple(reversed(heads)), tuple(reversed(depth))
+    for i, blk in enumerate(spec.up):
+        for j, (r, t) in enumerate(zip(blk.resnets, blk.attentions)):
+            spec.motion.append(motion(f"{blk.prefix}.motion_modules.{j}", blk.cout, rheads[i], rdepth[i],
+                                      (t or r).prefix))
+    return spec
+
+
+def motion_pe(max_seq_len, dim):
+    """diffusers ``SinusoidalPositionalEmbedding.pe`` [1, max_seq_len, dim]: sin on the even columns, cos on the odd
+    ones, frequencies exp(-2i ln(10000) / dim)."""
+    pos = torch.arange(max_seq_len, dtype=torch.float32).unsqueeze(1)
+    div = torch.exp(torch.arange(0, dim, 2, dtype=torch.float32) * (-math.log(10000.0) / dim))
+    pe = torch.zeros(1, max_seq_len, dim)
+    pe[0, :, 0::2] = torch.sin(pos * div)
+    pe[0, :, 1::2] = torch.cos(pos * div)
+    return pe
+
+
 _SVD_DOWN = ("CrossAttnDownBlockSpatioTemporal", "DownBlockSpatioTemporal")
 _SVD_UP = ("CrossAttnUpBlockSpatioTemporal", "UpBlockSpatioTemporal")
 
@@ -693,6 +824,21 @@ def param_shapes(spec: UNetSpec):
             conv(f"controlnet_down_blocks.{i}", c, c, 1)
         conv("controlnet_mid_block", spec.mid.cout, spec.mid.cout, 1)
         return out
+    for m in spec.motion:
+        norm(m.prefix + ".norm", m.dim)
+        lin(m.prefix + ".proj_in", m.dim, m.dim)
+        for d in range(m.depth):
+            b = f"{m.prefix}.transformer_blocks.{d}"
+            for a, n in (("attn1", "norm1"), ("attn2", "norm2")):
+                norm(f"{b}.{n}", m.dim)
+                for x in ("to_q", "to_k", "to_v"):
+                    lin(f"{b}.{a}.{x}", m.dim, m.dim, False)
+                lin(f"{b}.{a}.to_out.0", m.dim, m.dim)
+            norm(b + ".norm3", m.dim)
+            lin(b + ".ff.net.0.proj", m.dim * 8, m.dim)
+            lin(b + ".ff.net.2", m.dim, m.dim * 4)
+            out[b + ".pos_embed.pe"] = (1, m.max_seq_len, m.dim)  # a persistent buffer, not a parameter
+        lin(m.prefix + ".proj_out", m.dim, m.dim)
     norm("conv_norm_out", spec.block_out_channels[0])
     conv("conv_out", spec.out_channels, spec.block_out_channels[0], 3)
     if spec.ip is not None:
@@ -732,7 +878,9 @@ def random_state_dict(spec: UNetSpec, seed=0, dtype=torch.float16, device="cpu")
     sd = {}
     for name, shape in param_shapes(spec).items():
         is_norm = ".norm" in name or name.startswith("conv_norm_out")
-        if name.endswith("mix_factor"):
+        if name.endswith(".pos_embed.pe"):  # AnimateDiff's sinusoid buffer
+            t = motion_pe(shape[1], shape[2])
+        elif name.endswith("mix_factor"):
             t = torch.randn(shape, generator=g) * 1.5
         elif name.endswith(".latents"):  # IP-Adapter Plus queries, initialised as diffusers does
             t = torch.randn(shape, generator=g) / math.sqrt(shape[-1])
